@@ -16,30 +16,16 @@
 // blocks: Sᵀ = K·Qᵀ, dPᵀ = V·dOᵀ, dSᵀ = Pᵀ∘(dPᵀ − D), dV += Pᵀ·dO, dK += dSᵀ·Q; in the single-pass (fused) form the
 // same kernel stages dSᵀ in shared memory and reduces dQ += dS·K into an fp32 buffer with atomics.  The two-kernel form
 // computes dQ in a kernel of its own (CTA = 64 queries, loop over key blocks).
-#include "common.cuh"
+//
+// Which shapes run here: everything except the non-causal forward and single-pass backward with dh = 40 and N, M
+// multiples of 128 and >= 512 (the 4096-token self-attention), which the entry points below hand to the warpgroup
+// kernels of attention_wgmma.cu unless a switch (see "Runtime switches") keeps them here.
+#include "attention.cuh"
 #include <math.h>
 #include <stdlib.h>
 
-static constexpr float kLog2e = 1.4426950408889634f;
 static constexpr int kAttnThreads = 128;
 static constexpr int kBlk = 64;   // query rows of a forward / dQ CTA, key rows of a dK/dV CTA, key block of the loops
-
-struct AttnArgs {
-  int B, H, N, M, dh;
-  float scale;
-  int stages, lazy, poly, p_smem;   // forward variants (attn_fwd_kernel); stages is also the Q/dO buffering of the backward
-  const bf16* Q; long long ldq, q_bs;
-  const bf16* K; long long ldk, k_bs;
-  const bf16* V; long long ldv, v_bs;
-  bf16* O; long long ldo, o_bs;
-  const bf16* dO; long long lddo, do_bs;
-  float* LSE;        // [B][H][N]
-  const float* Dv;   // [B][H][N] rowsum(dO∘O)
-  float* dQacc;      // [B][N][H*dh] fp32 (fused backward)
-  bf16* dQ; long long lddq, dq_bs;
-  bf16* dK; long long lddk, dk_bs;
-  bf16* dV; long long lddv, dv_bs;
-};
 
 // rows [0, nrows) of a head slice -> smem [nrows][DP + 8]; rows >= rows_valid and columns >= dh are zero-filled
 template <int DP, int NT = kAttnThreads>
@@ -637,9 +623,20 @@ static int attn_dp(int dh) {
 //   E4T_ATTN_BWD_BQ    32: 32-query blocks in the dK/dV kernel for every head dim (default 64 for dh <= 96)
 //   E4T_ATTN_BWD_STAGES 1: Q / dO of the dK/dV loop single-buffered (default 2: next block prefetched)
 //   E4T_ATTN_BWD_FUSED 0: the non-causal single-pass entry point runs the two-kernel backward instead
+//   E4T_ATTN_WGMMA     0: the shapes of the warpgroup kernels (attention_wgmma.cu) run the mma.sync kernels of this file
+//                      instead.  Setting any of the kernel-variant switches above except E4T_ATTN_DELTA2 does the same:
+//                      they name variants of the mma.sync kernels.
 static int env_int(const char* name, int dflt) {
   const char* e = getenv(name);
   return (e && *e) ? atoi(e) : dflt;
+}
+
+static bool attn_use_wgmma(int N, int M, int dh) {
+  if (!attn_wgmma_shape_ok(N, M, dh) || !env_int("E4T_ATTN_WGMMA", 1)) return false;
+  for (const char* v : {"E4T_ATTN_FWD2", "E4T_ATTN_FWD_PT", "E4T_ATTN_CG", "E4T_ATTN_BWD_FUSED", "E4T_ATTN_BWD_BQ",
+                        "E4T_ATTN_BWD_STAGES"})
+    if (getenv(v)) return false;
+  return true;
 }
 
 static int attn_common_checks(int dh, long long ldq, long long ldk, long long ldv) {
@@ -689,6 +686,7 @@ extern "C" int e4t_attn_fwd(const void* Q, const void* K, const void* V, void* O
   if (int e = attn_common_checks(dh, ldq, ldk, ldv)) return e;
   AttnArgs a = attn_args(Q, K, V, B, H, N, M, dh, ldq, q_bs, ldk, k_bs, ldv, v_bs, scale);
   a.O = (bf16*)O; a.ldo = ldo; a.o_bs = o_bs; a.LSE = LSE;
+  if (attn_use_wgmma(N, M, dh)) return attn_wgmma_fwd(a, st);
   a.stages = 2;
   int warps = 4, cap = 0;
   if (const char* e = getenv("E4T_ATTN_FWD2")) {
@@ -753,6 +751,8 @@ static int attn_bwd_impl(const void* Q, const void* K, const void* V, const void
   const dim3 gkv(cdiv(M, kBlk), H, B), gq(cdiv(N, kBlk), H, B);
   const int dp = attn_dp(dh);
   int r = -1;
+  const bool wg = fused && !causal && attn_use_wgmma(N, M, dh);
+  if (wg) r = attn_wgmma_bwd(a, st);
 #define E4T_BWD_KV(D, BQ, S)                                                                                     \
   {                                                                                                              \
     const size_t skv = BwdCfg<D, BQ>::smem_bytes(fused);                                                         \
@@ -767,7 +767,7 @@ static int attn_bwd_impl(const void* Q, const void* K, const void* V, const void
     else E4T_BWD_KV(D, BQ, 1)                                                                                    \
   }
 #define E4T_BWD(D)                                                                                               \
-  if (dp == D) {                                                                                                 \
+  if (!wg && dp == D) {                                                                                               \
     if (D <= 96 && !bq32) E4T_BWD_BQ(D, (D <= 96 ? 64 : 32))                                                      \
     else E4T_BWD_BQ(D, 32)                                                                                       \
   }

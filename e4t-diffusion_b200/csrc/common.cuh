@@ -127,6 +127,14 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* m, ui
       : "memory");
 }
 
+// contiguous global -> shared copy (16-byte aligned, bytes % 16 == 0), mbarrier completion
+__device__ __forceinline__ void bulk_load_1d(void* smem, const void* g, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   smem_u32(smem)),
+               "l"(g), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+
 // ---- TMA stores (smem -> global, bulk async group completion) ------------------------------------
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
@@ -172,6 +180,16 @@ template <int R>
 __device__ __forceinline__ void reg_fence(float* d) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// the same for bf16-packed A-operand registers of a register-A wgmma, which the instruction reads until it retires
+template <int R>
+__device__ __forceinline__ void reg_fence_u32(uint32_t* a) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
+// named barrier over `nthreads` threads of the CTA (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 // warpgroup register re-allocation (producer warpgroup gives registers to the MMA warpgroups)
 template <int R>

@@ -296,7 +296,9 @@ def _bs(t):
 
 def attn_fwd(q, k, v, heads, scale=None):
     """q (B,N,H*dh), k/v (B,M,H*dh) bf16 (last dim contiguous; may be column slices of a fused projection).
-    Returns (o (B,N,H*dh) bf16, lse (B,H,N) fp32)."""
+    Returns (o (B,N,H*dh) bf16, lse (B,H,N) fp32).
+    dh == 40 with N and M multiples of 128, >= 512 (the 4096-token self-attention) runs the warpgroup (wgmma + TMA)
+    kernel; every other shape, or E4T_ATTN_WGMMA=0, the mma.sync kernel."""
     assert q.dtype == BF16 and k.dtype == BF16 and v.dtype == BF16
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1
     Bn, N, C = q.shape
@@ -314,7 +316,9 @@ def attn_fwd(q, k, v, heads, scale=None):
 def attn_bwd(q, k, v, o, do, lse, heads, scale=None, dq=None, dk=None, dv=None, fused=True, causal=False):
     """dq/dk/dv may be preallocated (e.g. column slices of one fused (B,N,3C) gradient buffer).
     fused=True: single-pass backward (S/dP computed once per tile pair, dQ reduced in fp32) when dh <= 80 and N >= 128;
-    otherwise / fused=False the two-kernel (dK/dV, dQ) path.
+    otherwise / fused=False the two-kernel (dK/dV, dQ) path.  The single-pass backward of a non-causal call with
+    dh == 40 and N, M multiples of 128, >= 512 runs the warpgroup (wgmma + TMA) kernel, which reduces dQ with bulk
+    tensor adds instead of scalar atomics; every other shape, or E4T_ATTN_WGMMA=0, the mma.sync kernel.
     causal=True (N == M, dh <= 80): key j contributes to query i only if j <= i; o / lse must come from a forward that
     applied the same mask (attn_small_fwd)."""
     assert do.dtype == BF16 and do.stride(-1) == 1
