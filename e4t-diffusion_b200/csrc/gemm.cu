@@ -12,8 +12,10 @@
 // Structure (per CTA, 384 threads = 3 warpgroups): warpgroup 0 is the TMA producer (one thread issues), warpgroups 1
 // and 2 each own 64 rows of the 128 x BN output tile and issue wgmma.m64nBNk16 from the shared-memory ring of `stages`
 // {A 128x64, B BNx64} bf16 tiles (SWIZZLE_128B).  The accumulator lives in registers; the epilogue (alpha, bias,
-// row-group addend, residual, bf16 / fp32 / fp32-atomic output) runs from registers while the producer already
-// fills the ring for the next tile.
+// row-group addend, residual) writes each warpgroup's 64 x BN result into its own shared-memory staging buffer, from
+// which TMA stores it (bf16 / fp32) or adds it (fp32 atomic mode) while the warpgroup already runs the next tile's
+// MMAs.  Outputs TMA cannot address (base, row pitch or batch stride not a multiple of 16 bytes) take a register
+// epilogue that stores from the accumulator fragments directly.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include <stdlib.h>
@@ -35,14 +37,19 @@ struct GemmArgs {
   const bf16* residual;  // [M][ldr] bf16 or null
   long long ldr, res_bstride;
   float alpha;
-  int pair_store;  // output rows and base allow two-element (4 / 8-byte) stores
-  int epi_plain;   // default on (E4T_GEMM_EPI_PLAIN=0 disables): lean loop for bf16 outputs with at most a bias
+  int pair_store;  // register epilogue: output rows and base allow two-element (4 / 8-byte) stores
+  int epi_tma;     // output staged in shared memory and written by TMA (mapO); 0 = register epilogue
 };
 
 static constexpr int kBM = 128;
 static constexpr int kBK = 64;
 static constexpr int kATileBytes = kBM * kBK * 2;  // 16 KiB
 static constexpr int kThreads = 384;               // producer warpgroup + 2 MMA / epilogue warpgroups
+// Output staging: each MMA warpgroup owns a 64 x BN bf16-sized buffer (fp32 outputs go through it in two column
+// halves), cut into 64-row x 64-byte sub-tiles in the SWIZZLE_64B layout, one TMA box each (32 bf16 / 16 fp32 columns).
+static constexpr int kSubBytes = 64 * 64;
+template <int BN>
+constexpr int kStgBytes = 64 * BN * 2;  // per warpgroup
 
 __device__ __forceinline__ void gemm_decode(const GemmArgs& g, long t, int& n_t, int& m_t, int& sp, int& bz) {
   n_t = (int)(t % g.n_tiles);
@@ -98,53 +105,89 @@ __device__ __forceinline__ void gemm_epilogue(const GemmArgs& g, const float* ac
   }
 }
 
-// Lean epilogue for the common case (QKV projections, every dX GEMM, bias-only linears): bf16 output, no alpha, row-group
-// addend or residual, pairs storable; the bias test is hoisted out of the column loop.  Same arithmetic as
-// gemm_epilogue, so both give bit-identical results.
-template <int BN, bool BIAS>
-__device__ __forceinline__ void gemm_epilogue_plain(const GemmArgs& g, const float* acc, int m_t, int n0, int bz,
-                                                    int wg_row) {
-  const int lane = threadIdx.x & 31;
-  const int w = (threadIdx.x >> 5) & 3;
+// Staged epilogue: the warpgroup applies alpha, bias, row-group addend and residual exactly as gemm_epilogue does,
+// writes its 64 x BN rows into its staging buffer, and one thread hands the buffer to TMA (a tile store, or a tile add
+// for the fp32-atomic mode).  The stores drain while the warpgroup runs the next tile's MMAs; the buffer is rewritten
+// only after TMA has read it.  Rows past M and columns past N are clipped by TMA.
+// Staging layout: sub-tile s holds columns [s * kSubCols, (s + 1) * kSubCols) as 64 rows of 64 bytes; the 16-byte chunk
+// c of row r sits at chunk c ^ ((r >> 1) & 3) (SWIZZLE_64B), so the 8 rows a warp writes per instruction hit 8
+// different bank groups.
+template <int BN, typename OutT>
+__device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUtensorMap* mapO, const float* acc,
+                                                  uint8_t* stg, int m_t, int n0, int bz, int wg_row, uint32_t bar_id) {
+  constexpr int kEsz = (int)sizeof(OutT);
+  constexpr int kSubCols = 64 / kEsz;  // 64-byte sub-tile rows: 32 bf16 or 16 fp32 columns
+  constexpr int kSubsPerPass = kStgBytes<BN> / kSubBytes;
+  constexpr int kPasses = BN / kSubCols / kSubsPerPass;  // 1 for bf16, 2 for fp32
+  const int tid = threadIdx.x & 127;
+  const int lane = tid & 31;
+  const int w = tid >> 5;
+  const int row0 = m_t * kBM + wg_row;
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int m = m_t * kBM + wg_row + w * 16 + (lane >> 2) + 8 * h;
-    if (m >= g.M) continue;
-    bf16* orow = reinterpret_cast<bf16*>(g.out) + (long long)bz * g.out_bstride + (long long)m * g.ldo;
+  for (int p = 0; p < kPasses; ++p) {
+    if (tid == 0) tma_store_wait_read<0>();
+    named_bar_sync(bar_id, 128);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int n = n0 + 8 * j + 2 * (lane & 3);
-      if (n >= g.N) break;
-      float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-      if (n + 1 < g.N) {
-        if (BIAS) {
-          f0 += g.bias[n];
-          f1 += g.bias[n + 1];
+    for (int h = 0; h < 2; ++h) {
+      const int r = w * 16 + (lane >> 2) + 8 * h;
+      const int m = row0 + r;
+      if (m >= g.M) continue;
+      const float* rg = g.rowgroup ? g.rowgroup + (long long)(m / g.rows_per_group) * g.N : nullptr;
+      const bf16* res = g.residual ? g.residual + (long long)bz * g.res_bstride + (long long)m * g.ldr : nullptr;
+      uint8_t* srow = stg + r * 64;
+      const int sw = (r >> 1) & 3;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int sub = 8 * j / kSubCols;
+        if (sub / kSubsPerPass != p) continue;
+        const int n = n0 + 8 * j + 2 * (lane & 3);
+        float f0 = acc[4 * j + 2 * h] * g.alpha, f1 = acc[4 * j + 2 * h + 1] * g.alpha;
+        if (n < g.N) {
+          const bool two = n + 1 < g.N;
+          if (g.bias) { f0 += g.bias[n]; if (two) f1 += g.bias[n + 1]; }
+          if (rg) { f0 += rg[n]; if (two) f1 += rg[n + 1]; }
+          if (res) { f0 += __bfloat162float(res[n]); if (two) f1 += __bfloat162float(res[n + 1]); }
         }
-        *reinterpret_cast<uint32_t*>(orow + n) = pack_bf16(f0, f1);
-      } else {
-        if (BIAS) f0 += g.bias[n];
-        orow[n] = __float2bfloat16(f0);
+        const int byte = (8 * j % kSubCols + 2 * (lane & 3)) * kEsz;
+        uint8_t* dst = srow + (sub % kSubsPerPass) * kSubBytes + ((((byte >> 4) ^ sw)) << 4) + (byte & 15);
+        if (kEsz == 2) *reinterpret_cast<uint32_t*>(dst) = pack_bf16(f0, f1);
+        else *reinterpret_cast<float2*>(dst) = make_float2(f0, f1);
       }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(bar_id, 128);
+    if (tid == 0 && row0 < g.M) {
+#pragma unroll 1
+      for (int s = 0; s < kSubsPerPass; ++s) {
+        const int n = n0 + (p * kSubsPerPass + s) * kSubCols;
+        if (n >= g.N) break;
+        if (g.out_mode == 2) tma_reduce_add_3d(mapO, stg + s * kSubBytes, n, row0, bz);
+        else tma_store_3d(mapO, stg + s * kSubBytes, n, row0, bz);
+      }
+      tma_store_commit();
     }
   }
 }
 
 template <int BN, int AMN, int BMN>
 __global__ void __launch_bounds__(kThreads, 1)
-e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const GemmArgs g) {
+e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                const __grid_constant__ CUtensorMap mapO, const GemmArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // align dynamic smem to 1024 B (SWIZZLE_128B atoms)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   constexpr int kBTileBytes = BN * kBK * 2;
   constexpr int kStageBytes = kATileBytes + kBTileBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)g.stages * kStageBytes);
+  // [stages x {A, B}] [staging of MMA warpgroup 0] [staging of MMA warpgroup 1] [full / empty barriers]
+  uint8_t* staging = smem + (size_t)g.stages * kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + 2 * kStgBytes<BN>);
   uint64_t* empty_bar = full_bar + g.stages;
 
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
+    if (g.epi_tma) tma_prefetch_desc(&mapO);
     for (int i = 0; i < g.stages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 256);
@@ -262,13 +305,16 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
       wgmma_wait<0>();
       reg_fence<BN / 2>(acc);
       if (prev >= 0) mbar_arrive(&empty_bar[prev]);
-      if (g.epi_plain && g.out_mode == 0 && g.alpha == 1.f && !g.rowgroup && !g.residual && g.pair_store) {
-        if (g.bias) gemm_epilogue_plain<BN, true>(g, acc, m_t, n_t * BN, bz, wg_row);
-        else gemm_epilogue_plain<BN, false>(g, acc, m_t, n_t * BN, bz, wg_row);
-      } else {
+      if (!g.epi_tma) {
         gemm_epilogue<BN, AMN, BMN>(g, acc, m_t, n_t * BN, bz, wg_row);
+      } else {
+        uint8_t* stg = staging + (wg - 1) * kStgBytes<BN>;
+        if (g.out_mode == 0) gemm_epilogue_tma<BN, bf16>(g, &mapO, acc, stg, m_t, n_t * BN, bz, wg_row, wg);
+        else gemm_epilogue_tma<BN, float>(g, &mapO, acc, stg, m_t, n_t * BN, bz, wg_row, wg);
       }
     }
+    // shared memory must outlive the last TMA reads of the staging buffer
+    if (g.epi_tma && (threadIdx.x & 127) == 0) tma_store_wait_all();
   }
 }
 
@@ -288,12 +334,15 @@ static int num_sms() {
 
 // Tile-width choice by a cost model in nominal cycles per CTA, with rates taken from the H100 SXM data sheet (989 dense
 // BF16 TFLOP/s over 132 SMs: a 128 x BN x 64 k-chunk is ~3.9 * BN cycles of tensor-core work) plus a fixed per-chunk
-// hand-off cost; the register epilogue writes each output element once (fp32 atomics cost several times a store):
+// hand-off cost; the epilogue term was fitted to the register epilogue, which wrote each output element once (fp32
+// atomics cost several times a store):
 //   mainloop per 64-deep k-chunk  = 160 + 3.9 * BN
 //   epilogue per tile             = 600 + 12 * BN * (1 + [residual]) * (4 if fp32 atomics)
-//   kernel                        = ceil(tiles / SMs) * (mainloop + epilogue)   (the producer runs ahead, the
-//                                                                                 epilogue is not overlapped)
-// The widest tile that does not add a round of the persistent grid wins; wide tiles also halve operand traffic.
+//   kernel                        = ceil(tiles / SMs) * (mainloop + epilogue)
+// The staged epilogue's TMA stores drain under the next tile's MMAs, so the epilogue term now overstates what a tile
+// pays; it is kept until it is refitted to measured staged-epilogue timings, since a rough repricing moves the split-K
+// factor of the large weight gradients.  The widest tile that does not add a round of the persistent grid wins; wide
+// tiles also halve operand traffic.
 static int pick_bn(int N, long m_tiles_x_batch, bool b_mn, int force_bn, int kchunks_per_tile = 16,
                    bool residual = false, bool atomic = false, double* cost_out = nullptr) {
   if (force_bn > 0) return force_bn;
@@ -337,38 +386,41 @@ static int auto_splits(int N, long m_tiles_x_batch, bool b_mn, int kchunks) {
 }
 
 template <int BN, int AMN, int BMN>
-static int launch_gemm_t(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs& g, int grid, cudaStream_t stream) {
+static int launch_gemm_t(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, GemmArgs& g, int grid,
+                         cudaStream_t stream) {
   constexpr int stage_bytes = kATileBytes + BN * kBK * 2;
-  int stages = (200 * 1024) / stage_bytes;
+  // the ring gets what the two staging buffers, the barriers and the 1 KiB alignment slack leave of 227 KiB
+  int stages = (227 * 1024 - 1024 - 2 * kStgBytes<BN> - 16 * (int)sizeof(uint64_t)) / stage_bytes;
   if (stages > 8) stages = 8;
   if (stages > g.kper) stages = g.kper < 2 ? 2 : g.kper;
   g.stages = stages;
-  const size_t smem = (size_t)stages * stage_bytes + 2 * stages * sizeof(uint64_t) + 1024;
+  const size_t smem = (size_t)stages * stage_bytes + 2 * kStgBytes<BN> + 2 * stages * sizeof(uint64_t) + 1024;
   static bool attr_set = false;
   if (!attr_set) {
     E4T_CUDA(cudaFuncSetAttribute(e4t_gemm_kernel<BN, AMN, BMN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   227 * 1024));
     attr_set = true;
   }
-  e4t_gemm_kernel<BN, AMN, BMN><<<grid, kThreads, smem, stream>>>(mA, mB, g);
+  e4t_gemm_kernel<BN, AMN, BMN><<<grid, kThreads, smem, stream>>>(mA, mB, mO, g);
   E4T_COUNT_LAUNCH();
   E4T_LAUNCH_CHECK();
   return 0;
 }
 
 template <int AMN, int BMN>
-static int launch_gemm_bn(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs& g, int grid, cudaStream_t stream) {
+static int launch_gemm_bn(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, GemmArgs& g, int grid,
+                          cudaStream_t stream) {
   switch (g.BN) {
-    case 64: return launch_gemm_t<64, AMN, BMN>(mA, mB, g, grid, stream);
-    case 128: return launch_gemm_t<128, AMN, BMN>(mA, mB, g, grid, stream);
-    case 192: return launch_gemm_t<192, AMN, BMN>(mA, mB, g, grid, stream);
-    case 256: return launch_gemm_t<256, AMN, BMN>(mA, mB, g, grid, stream);
+    case 64: return launch_gemm_t<64, AMN, BMN>(mA, mB, mO, g, grid, stream);
+    case 128: return launch_gemm_t<128, AMN, BMN>(mA, mB, mO, g, grid, stream);
+    case 192: return launch_gemm_t<192, AMN, BMN>(mA, mB, mO, g, grid, stream);
+    case 256: return launch_gemm_t<256, AMN, BMN>(mA, mB, mO, g, grid, stream);
   }
   if (!BMN) {
     switch (g.BN) {
-      case 96: return launch_gemm_t<96, AMN, 0>(mA, mB, g, grid, stream);
-      case 160: return launch_gemm_t<160, AMN, 0>(mA, mB, g, grid, stream);
-      case 224: return launch_gemm_t<224, AMN, 0>(mA, mB, g, grid, stream);
+      case 96: return launch_gemm_t<96, AMN, 0>(mA, mB, mO, g, grid, stream);
+      case 160: return launch_gemm_t<160, AMN, 0>(mA, mB, mO, g, grid, stream);
+      case 224: return launch_gemm_t<224, AMN, 0>(mA, mB, mO, g, grid, stream);
     }
   }
   return e4t_set_error("e4t_gemm_bf16: unsupported tile width BN=%d (b_mn=%d)", g.BN, BMN);
@@ -376,17 +428,29 @@ static int launch_gemm_bn(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs
 
 static int launch_gemm(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs& g, cudaStream_t stream) {
   const int esz = g.out_mode == 0 ? 2 : 4;
-  {
-    const char* p = getenv("E4T_GEMM_EPI_PLAIN");
-    g.epi_plain = (p && *p) ? atoi(p) : 1;
-  }
   g.pair_store = (g.ldo % 2) == 0 && (g.batch == 1 || (g.out_bstride % 2) == 0) && ((uintptr_t)g.out % (2 * esz)) == 0;
+  // TMA addresses the output when its base is 16-byte aligned and its row pitch and batch stride are multiples of
+  // 16 bytes; anything else, or E4T_GEMM_EPI_PLAIN=0, takes the register epilogue.
+  const char* p = getenv("E4T_GEMM_EPI_PLAIN");
+  const bool want_tma = !(p && *p) || atoi(p) != 0;
+  g.epi_tma = want_tma && ((uintptr_t)g.out % 16) == 0 && (g.ldo * esz) % 16 == 0 && g.ldo >= g.N &&
+              (g.batch == 1 || (g.out_bstride > 0 && (g.out_bstride * esz) % 16 == 0));
+  CUtensorMap mO;
+  memset(&mO, 0, sizeof(mO));
+  if (g.epi_tma) {
+    const uint64_t bs = g.batch == 1 ? (uint64_t)g.ldo * g.M : (uint64_t)g.out_bstride;
+    uint64_t dims[3] = {(uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.batch};
+    uint64_t str[2] = {(uint64_t)g.ldo * esz, bs * esz};
+    uint32_t box[3] = {(uint32_t)(64 / esz), 64, 1};
+    if (int e = e4t_tmap_encode(&mO, g.out, 3, dims, str, box, esz, 64)) return e;
+  }
   const long total = (long)g.batch * g.splits * g.m_tiles * g.n_tiles;
   int grid = (int)(total < num_sms() ? total : num_sms());
   if (grid < 1) return 0;
   // the implicit convolutions load A K-major (wgrad: both operands MN-major, set in a_mn / b_mn)
-  if (g.a_mn) return g.b_mn ? launch_gemm_bn<1, 1>(mA, mB, g, grid, stream) : launch_gemm_bn<1, 0>(mA, mB, g, grid, stream);
-  return g.b_mn ? launch_gemm_bn<0, 1>(mA, mB, g, grid, stream) : launch_gemm_bn<0, 0>(mA, mB, g, grid, stream);
+  if (g.a_mn)
+    return g.b_mn ? launch_gemm_bn<1, 1>(mA, mB, mO, g, grid, stream) : launch_gemm_bn<1, 0>(mA, mB, mO, g, grid, stream);
+  return g.b_mn ? launch_gemm_bn<0, 1>(mA, mB, mO, g, grid, stream) : launch_gemm_bn<0, 0>(mA, mB, mO, g, grid, stream);
 }
 
 extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, int batch, int a_mn,
