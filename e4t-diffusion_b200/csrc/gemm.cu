@@ -27,6 +27,7 @@ struct GemmArgs {
   // implicit 3x3 convolution (conv = 1: forward / dgrad, 2: weight gradient)
   int conv, H, W, BH, BB, cin_chunks, cout;
   int cstride;   // spatial stride of the forward convolution (1, or 2 = Downsample2D; H, W are the OUTPUT size)
+  int cpad;      // top / left zero padding of the forward convolution (1; or 0 = diffusers Downsample2D(padding=0))
   // epilogue
   void* out;
   int out_mode;  // 0 = bf16 store, 1 = fp32 store, 2 = fp32 atomic add
@@ -210,11 +211,12 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
       const int m0 = m_t * kBM, n0 = n_t * BN;
       const int kc0 = sp * g.kper;
       const int kc1 = min(g.kchunks, kc0 + g.kper);
-      int cb0 = 0, ch0 = 0;
+      int cb0 = 0, ch0 = 0, cw0 = 0;
       if (g.conv == 1) {
         const int img = g.H * g.W;
         cb0 = m0 / img;
         ch0 = (m0 % img) / g.W;
+        cw0 = m0 % g.W;  // non-zero only for rows wider than a tile (W > 128: a tile is 128 pixels of one row)
       }
       for (int kc = kc0; kc < kc1; ++kc) {
         mbar_wait(&empty_bar[s], ph ^ 1u);
@@ -235,7 +237,8 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         } else if (g.conv) {
           const int tap = kc / g.cin_chunks, cc = kc % g.cin_chunks;
           const int dy = tap / 3, dx = tap % 3;
-          tma_load_4d(sA, &mapA, &full_bar[s], cc * kBK, dx - 1, g.cstride * ch0 + dy - 1, cb0);
+          tma_load_4d(sA, &mapA, &full_bar[s], cc * kBK, g.cstride * cw0 + dx - g.cpad, g.cstride * ch0 + dy - g.cpad,
+                      cb0);
           tma_load_2d(sB, &mapB, &full_bar[s], cc * kBK, tap * g.cout + n0);
         } else {
           const int ab = g.a_batched ? bz : 0, bb = g.b_batched ? bz : 0;
@@ -519,21 +522,34 @@ extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int
 }
 
 // x: NHWC bf16 [B][Hin][Win][Cin];  w: bf16 [9][Cout][Cin] (tap = ky*3+kx);  out: [B*H*W][Cout] (NHWC), H = Hin/stride.
-// pad 1.  bias fp32 [Cout]; rowgroup fp32 [B][Cout] (time-embedding projection) ; residual bf16 NHWC.
+// bias fp32 [Cout]; rowgroup fp32 [B][Cout] (time-embedding projection) ; residual bf16 NHWC.
+// Padding: pad_lo zero rows / columns on the top and left (1 = the symmetric pad-1 convolution); the taps of output
+// pixel (y, x) read input (stride*y + ky - pad_lo, stride*x + kx - pad_lo), and whatever falls outside the input, on
+// either side, is TMA out-of-bounds zero fill.  pad_lo = 0 with stride 2 is diffusers' Downsample2D(padding=0), which
+// pads one zero row / column on the bottom and right only.
 // stride 2 (diffusers Downsample2D): the A-operand tensor map walks the input with element strides (1,2,2,1), so the
 // tile of 128 OUTPUT pixels is gathered directly from every other input pixel — no stride-1 result is computed and
 // thrown away (round 1 did exactly that: 4x the FLOPs on the three downsampling convolutions).
+// Tiles: an output width W that divides 128 gives tiles of 128 / W whole rows (or whole images when H*W < 128); a
+// width W > 128 that is a multiple of 128 gives tiles of 128 consecutive pixels of one row, whose first column the
+// producer adds to the A-operand x coordinate.
 static int conv3x3_impl(const void* x, const void* w, void* out, int B, int Hin, int Win, int Cin, int Cout, int stride,
-                        int out_mode, const float* bias, const float* rowgroup, const void* residual, int force_bn,
-                        cudaStream_t stream) {
+                        int pad_lo, int out_mode, const float* bias, const float* rowgroup, const void* residual,
+                        int force_bn, cudaStream_t stream) {
   E4T_CHECK(Cin % 64 == 0, "e4t_conv3x3: Cin must be a multiple of 64 (got %d)", Cin);
   E4T_CHECK(stride == 1 || (stride == 2 && Hin % 2 == 0 && Win % 2 == 0), "e4t_conv3x3: bad stride/size");
+  E4T_CHECK(pad_lo == 1 || (stride == 2 && pad_lo == 0), "e4t_conv3x3: bad padding %d for stride %d", pad_lo, stride);
   const int H = Hin / stride, W = Win / stride;
-  E4T_CHECK(W <= 128 && (128 % W) == 0, "e4t_conv3x3: output width must divide 128 (got %d)", W);
+  const bool wide = W > 128;
+  E4T_CHECK((W <= 128 && (128 % W) == 0) || (wide && W % 128 == 0),
+            "e4t_conv3x3: output width must divide 128 or be a multiple of 128 (got %d)", W);
   E4T_CHECK(out_mode == 0 || out_mode == 1, "e4t_conv3x3: bad out_mode");
   const int img = H * W;
   int BH, BB;
-  if (img >= 128) {
+  if (wide) {
+    BB = 1;
+    BH = 1;
+  } else if (img >= 128) {
     BB = 1;
     BH = 128 / W;
     E4T_CHECK(H % BH == 0, "e4t_conv3x3: H=%d not a multiple of tile height %d", H, BH);
@@ -542,10 +558,12 @@ static int conv3x3_impl(const void* x, const void* w, void* out, int B, int Hin,
     BB = 128 / img;
     BH = H;
   }
+  const int BW = wide ? 128 : W;
   GemmArgs g;
   memset(&g, 0, sizeof(g));
   g.M = B * img; g.N = Cout; g.K = Cin; g.batch = 1;
   g.conv = 1; g.H = H; g.W = W; g.BH = BH; g.BB = BB; g.cin_chunks = Cin / 64; g.cout = Cout; g.cstride = stride;
+  g.cpad = pad_lo;
   g.m_tiles = cdiv(g.M, kBM);
   g.kchunks = 9 * g.cin_chunks;
   g.kper = g.kchunks; g.splits = 1;
@@ -559,7 +577,7 @@ static int conv3x3_impl(const void* x, const void* w, void* out, int B, int Hin,
   {
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)Win, (uint64_t)Hin, (uint64_t)B};
     uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)Win * Cin * 2, (uint64_t)Hin * Win * Cin * 2};
-    uint32_t box[4] = {kBK, (uint32_t)(W * stride), (uint32_t)(BH * stride), (uint32_t)BB};
+    uint32_t box[4] = {kBK, (uint32_t)(BW * stride), (uint32_t)(BH * stride), (uint32_t)BB};
     uint32_t es[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
     if (int e = e4t_tmap_encode(&mA, x, 4, dims, str, box, 2, 128, stride == 1 ? nullptr : es)) return e;
   }
@@ -575,7 +593,7 @@ static int conv3x3_impl(const void* x, const void* w, void* out, int B, int Hin,
 extern "C" int e4t_conv3x3_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                                 int out_mode, const float* bias, const float* rowgroup, const void* residual,
                                 int force_bn, void* stream_) {
-  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 1, out_mode, bias, rowgroup, residual, force_bn,
+  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 1, 1, out_mode, bias, rowgroup, residual, force_bn,
                       (cudaStream_t)stream_);
 }
 
@@ -583,7 +601,15 @@ extern "C" int e4t_conv3x3_bf16(const void* x, const void* w, void* out, int B, 
 // out [B][H/2][W/2][Cout].
 extern "C" int e4t_conv3x3_s2_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                                    const float* bias, int force_bn, void* stream_) {
-  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 2, 0, bias, nullptr, nullptr, force_bn, (cudaStream_t)stream_);
+  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 2, 1, 0, bias, nullptr, nullptr, force_bn, (cudaStream_t)stream_);
+}
+
+// 3x3 / stride 2 with pad_lo zero rows / columns on the top and left: pad_lo = 1 is e4t_conv3x3_s2_bf16; pad_lo = 0 is
+// diffusers' Downsample2D(padding=0) (F.pad(x, (0, 1, 0, 1)) then an unpadded stride-2 convolution; the VAE encoder).
+extern "C" int e4t_conv3x3_s2p_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
+                                    int pad_lo, const float* bias, int force_bn, void* stream_) {
+  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 2, pad_lo, 0, bias, nullptr, nullptr, force_bn,
+                      (cudaStream_t)stream_);
 }
 
 // 3x3 / stride 1 / pad 1 weight gradient: dw9[tap][co][ci] += sum_{b,y,x} dy[b][y][x][co] * x[b][y+ky-1][x+kx-1][ci]
@@ -601,7 +627,7 @@ extern "C" int e4t_conv3x3_wgrad(const void* x, const void* dy, float* dw9, int 
   memset(&g, 0, sizeof(g));
   g.M = Cout; g.N = Cin; g.K = (int)pixels; g.batch = 9;
   g.a_mn = 1; g.b_mn = 1; g.a_batched = 0; g.b_batched = 1;
-  g.conv = 2; g.H = H; g.W = W; g.cout = Cout; g.cstride = 1;
+  g.conv = 2; g.H = H; g.W = W; g.cout = Cout; g.cstride = 1; g.cpad = 1;
   g.m_tiles = cdiv(Cout, kBM);
   g.kchunks = (int)(pixels / kBK);
   // enough K-splits to fill the machine about twice: tiles = 9 taps x m_tiles x n_tiles x splits

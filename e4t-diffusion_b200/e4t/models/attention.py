@@ -1,6 +1,8 @@
 """BasicTransformerBlock / FeedForward / GEGLU — mirror of e4t/models/attention.py:181-430 on the sm_90a kernels.
 LayerNorm -> attn1 (self) -> LayerNorm -> attn2 (cross) -> LayerNorm -> GEGLU feed-forward, residual adds fused into
-the producing GEMM epilogues."""
+the producing GEMM epilogues.  AttentionBlock (attention.py:37-178): the VAE mid-block's single-head attention,
+forward only."""
+import math
 from typing import Optional
 
 import torch
@@ -75,3 +77,67 @@ class BasicTransformerBlock(nn.Module):
             x = self.attn2(self._ln(self.norm2, x), encoder_hidden_states=encoder_hidden_states,
                            attention_mask=attention_mask, residual=x, **kw)                # :304-316
         return self.ff(self._ln(self.norm3, x), residual=x)                                # :318-330
+
+
+# the fp32 score matrix of one image is N² · 4 bytes (64 MiB at a 64 x 64 latent); images are processed in chunks
+# whose scores stay under this bound
+ATTN_SCORE_BYTES = 1 << 30
+
+
+class AttentionBlock(nn.Module):
+    """attention.py:37-178 — the single-head spatial self-attention of the VAE mid-block (diffusers 0.14, forward only).
+    GroupNorm (no SiLU) -> q|k|v as ONE GEMM with bias (weights row-concatenated) -> S = scale·Q·Kᵀ in fp32 (batched
+    GEMM) -> row softmax to bf16 -> O = P·V (V MN-major) -> proj_attn with bias and the residual in the epilogue.
+    The reference order of operations (:152-177): scores in the working dtype, softmax in fp32, (h + residual) / 1."""
+
+    def __init__(self, channels: int, num_head_channels: Optional[int] = None, norm_num_groups: int = 32,
+                 rescale_output_factor: float = 1.0, eps: float = 1e-5):
+        super().__init__()
+        self.channels = channels
+        self.num_heads = channels // num_head_channels if num_head_channels is not None else 1
+        self.num_head_size = num_head_channels
+        self.group_norm = nn.GroupNorm(num_channels=channels, num_groups=norm_num_groups, eps=eps, affine=True)
+        self.query = nn.Linear(channels, channels)
+        self.key = nn.Linear(channels, channels)
+        self.value = nn.Linear(channels, channels)
+        self.rescale_output_factor = rescale_output_factor
+        self.proj_attn = nn.Linear(channels, channels, 1)
+
+    def _qkv(self):
+        """q|k|v weights row-concatenated into one bf16 GEMM operand + fp32 bias; cached on query's parameters and
+        keyed on the versions and storage of key's and value's, so an update of any of the three rebuilds them."""
+        ps = (self.query, self.key, self.value)
+        kv = lambda n: tuple((getattr(p, n)._version, getattr(p, n).data_ptr()) for p in ps[1:])
+        w = FN.prepared(self.query.weight, ("vae_qkv_w",) + kv("weight"),
+                        lambda _: torch.cat([p.weight.detach() for p in ps], 0).to(torch.bfloat16).contiguous())
+        b = FN.prepared(self.query.bias, ("vae_qkv_b",) + kv("bias"),
+                        lambda _: torch.cat([p.bias.detach() for p in ps], 0).float().contiguous())
+        return w, b
+
+    def forward(self, hidden_states):
+        """hidden_states: channels-last (B, H, W, C) bf16 CUDA tensor."""
+        if self.num_heads != 1 or self.rescale_output_factor != 1.0:
+            raise NotImplementedError("only the single-head, unscaled AttentionBlock of the VAE is supported")
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise NotImplementedError("AttentionBlock runs inference only (no backward)")
+        from e4t.models.resnet import f32
+        from e4t_b200 import ops
+        x = FN._c(FN.as_bf16(hidden_states))
+        B, H, W, C = x.shape
+        N = H * W
+        gn = self.group_norm
+        h = ops.groupnorm_fwd(x, f32(gn.weight), f32(gn.bias), gn.num_groups, gn.eps, False)[0]
+        w_qkv, b_qkv = self._qkv()
+        qkv = ops.gemm(h.view(B * N, C), w_qkv, bias=b_qkv).view(B, N, 3 * C)
+        scale = 1.0 / math.sqrt(C / self.num_heads)
+        o = torch.empty((B, N, C), device=x.device, dtype=torch.bfloat16)
+        chunk = max(1, ATTN_SCORE_BYTES // (N * N * 4))
+        for i in range(0, B, chunk):
+            q, k, v = qkv[i:i + chunk, :, :C], qkv[i:i + chunk, :, C:2 * C], qkv[i:i + chunk, :, 2 * C:]
+            s = ops.gemm(q, k, alpha=scale, out_dtype=torch.float32)               # (b, N, N) fp32
+            p = ops.softmax_rows(s)
+            del s
+            ops.gemm(p, v, b_mn=True, out=o[i:i + chunk])
+        w_o = FN.prepared(self.proj_attn.weight, "bf16", lambda t: t.to(torch.bfloat16).contiguous())
+        out = ops.gemm(o.view(B * N, C), w_o, bias=f32(self.proj_attn.bias), residual=x.view(B * N, C))
+        return out.view(B, H, W, C)

@@ -22,8 +22,14 @@ def conv_w9_dgrad(conv):
                        .to(torch.bfloat16).contiguous())
 
 
+def f32(p):
+    """fp32 view of a parameter the kernels read as fp32 (biases, norm affine): the parameter itself when it is fp32,
+    else a cached fp32 copy (a model cast to a lower weight dtype, e.g. the VAE under `vae.to(weight_dtype)`)."""
+    return p if p is None or p.dtype == torch.float32 else FN.prepared(p, "f32", lambda t: t.float().contiguous())
+
+
 def conv3x3(conv, x, rowgroup=None, residual=None):
-    return FN.Conv3x3Fn.apply(x, conv_w9(conv), conv_w9_dgrad(conv), conv.bias, rowgroup, residual, conv.weight)
+    return FN.Conv3x3Fn.apply(x, conv_w9(conv), conv_w9_dgrad(conv), f32(conv.bias), rowgroup, residual, conv.weight)
 
 
 class Upsample2D(nn.Module):
@@ -50,8 +56,8 @@ class Upsample2D(nn.Module):
 class Downsample2D(nn.Module):
     def __init__(self, channels, use_conv=False, out_channels=None, padding=1, name="conv"):
         super().__init__()
-        if not use_conv or padding != 1:
-            raise NotImplementedError("SD-v1.x uses 3x3 stride-2 pad-1 conv downsampling only")
+        if not use_conv or padding not in (0, 1):
+            raise NotImplementedError("only 3x3 stride-2 conv downsampling with padding 1 (UNet) or 0 (VAE) is supported")
         self.channels = channels
         self.out_channels = out_channels or channels
         self.padding = padding
@@ -65,6 +71,12 @@ class Downsample2D(nn.Module):
     def forward(self, hidden_states):
         # stride-2 convolution computed directly at the output resolution (SURVEY.md §8 a-9)
         c = self.conv
+        if self.padding == 0:
+            # diffusers pads one zero row / column on the bottom and right (F.pad(x, (0, 1, 0, 1))) and convolves without
+            # padding; the kernel reads those zeros as out-of-bounds fill.  Forward only (the VAE encoder is frozen).
+            if torch.is_grad_enabled() and (hidden_states.requires_grad or c.weight.requires_grad):
+                raise NotImplementedError("Downsample2D(padding=0) has no backward (the VAE runs inference only)")
+            return FN.ops.conv3x3_s2(FN._c(hidden_states), conv_w9(c), bias=f32(c.bias), pad_lo=0)
         return FN.Conv3x3S2Fn.apply(hidden_states, conv_w9(c), conv_w9_dgrad(c), c.bias, c.weight)
 
 
@@ -110,13 +122,13 @@ class ResnetBlock2D(nn.Module):
             raise NotImplementedError("output_scale_factor != 1")
         x = input_tensor
         n1, n2 = self.norm1, self.norm2
-        h = FN.GroupNormFn.apply(x, n1.weight, n1.bias, n1.num_groups, n1.eps, True)
+        h = FN.GroupNormFn.apply(x, f32(n1.weight), f32(n1.bias), n1.num_groups, n1.eps, True)
         h = conv3x3(self.conv1, h, rowgroup=self.temb_row(temb))
-        h = FN.GroupNormFn.apply(h, n2.weight, n2.bias, n2.num_groups, n2.eps, True)
+        h = FN.GroupNormFn.apply(h, f32(n2.weight), f32(n2.bias), n2.num_groups, n2.eps, True)
         if self.conv_shortcut is not None:
             B, H, W, C = x.shape
             w = FN.prepared(self.conv_shortcut.weight, "bf16_1x1",
                             lambda t: t.reshape(t.shape[0], t.shape[1]).to(torch.bfloat16).contiguous())
-            x = FN.LinearFn.apply(x.view(B, H * W, C), w, self.conv_shortcut.bias, None,
+            x = FN.LinearFn.apply(x.view(B, H * W, C), w, f32(self.conv_shortcut.bias), None,
                                   self.conv_shortcut.weight).view(B, H, W, -1)
         return conv3x3(self.conv2, h, residual=x)

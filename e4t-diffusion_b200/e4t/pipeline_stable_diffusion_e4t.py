@@ -15,8 +15,9 @@ instead of once per step (SURVEY.md §8 f-2).
 
 diffusers is not a dependency: the SD-v1.x DDIM scheduler (scaled-linear betas, steps_offset 1, no sample clipping,
 eta) is `DDIMScheduler` below; any object with set_timesteps / scale_model_input / step(...).prev_sample works.
-VAE decoding is outside SURVEY.md §8: with `vae=None` the pipeline returns latents (`output_type="latent"`); a
-user-supplied `vae` with `.decode(z).sample` is called as the reference does (decode_latents)."""
+VAE decoding (decode_latents) calls `vae.decode(z).sample` as the reference does: attach e4t's AutoencoderKL
+(e4t/models/autoencoder_kl.py, the SD VAE on the same sm_90a kernels) and `output_type="np"` / `"pil"` run end to end on
+them; with `vae=None` the pipeline can only return latents (`output_type="latent"`)."""
 from dataclasses import dataclass
 from typing import List, Optional, Union
 
@@ -110,7 +111,10 @@ class StableDiffusionE4TPipeline:
         with torch.no_grad():
             self.class_embed = text_encoder.get_input_embeddings()(ids.to(text_encoder.device))      # :60
         self.domain_embed_scale = e4t_config.domain_embed_scale
-        self.vae_scale_factor = 8
+        # latent-to-pixel factor of the VAE's downsampling levels (8 for the SD VAE); 8 without a VAE or for a VAE object
+        # that has no config.block_out_channels
+        boc = getattr(getattr(vae, "config", None), "block_out_channels", None)
+        self.vae_scale_factor = 2 ** (len(boc) - 1) if boc else 8
 
     @property
     def _execution_device(self):
@@ -144,7 +148,7 @@ class StableDiffusionE4TPipeline:
 
     def decode_latents(self, latents):
         if self.vae is None:
-            raise NotImplementedError("no VAE attached: use output_type='latent' (VAE decode is outside SURVEY.md §8)")
+            raise NotImplementedError("no VAE attached: use output_type='latent' or pass an AutoencoderKL as `vae`")
         image = self.vae.decode(latents / 0.18215).sample
         return (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).float().numpy()
 

@@ -166,8 +166,12 @@ class PretrainStep:
     def __init__(self, unet, e4t_encoder, text_encoder, placeholder_token_id, class_token_id, lr=1.6e-5,
                  betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, domain_embed_scale=0.1, reg_lambda=0.01,
                  bos_id=49406, eos_id=49407, weight_dtype=torch.bfloat16, optimizer=True, tune_unet=False,
-                 max_grad_norm=None):
+                 max_grad_norm=None, vae=None):
         self.unet, self.enc, self.text = unet, e4t_encoder, text_encoder
+        # vae: an e4t AutoencoderKL; with it, a batch without "latents" is encoded on the device (pretrain_e4t.py:598-599)
+        self.vae = vae
+        if vae is not None:
+            vae.requires_grad_(False)                                                    # :262
         self.placeholder_token_id = placeholder_token_id
         self.domain_embed_scale, self.reg_lambda = domain_embed_scale, reg_lambda
         self.weight_dtype = weight_dtype
@@ -221,8 +225,19 @@ class PretrainStep:
         """[ids.index(placeholder_id) for ids in input_ids] (pretrain_e4t.py:617) — exact integer bookkeeping."""
         return [row.index(self.placeholder_token_id) for row in input_ids.cpu().tolist()]
 
+    def encode_latents(self, pixel_values, vae_noise=None):
+        """vae.encode(pixel_values).latent_dist.sample() * scaling_factor (pretrain_e4t.py:598-599); the Gaussian noise is
+        `vae_noise` when given, else drawn on the device."""
+        with torch.no_grad():
+            post = self.vae.encode(pixel_values.to(self.vae.dtype)).latent_dist
+            return post.sample(noise=vae_noise) * self.vae.config.scaling_factor
+
     def forward_loss(self, batch):
-        pixel_values, latents, noise = batch["pixel_values"], batch["latents"], batch["noise"]
+        pixel_values, latents, noise = batch["pixel_values"], batch.get("latents"), batch["noise"]
+        if latents is None:
+            if self.vae is None:
+                raise KeyError("batch has no 'latents' and no VAE is attached to encode 'pixel_values'")
+            latents = self.encode_latents(pixel_values, batch.get("vae_noise"))
         timesteps, input_ids = batch["timesteps"], batch["input_ids"]
         B = latents.shape[0]
         emb = self.text.get_input_embeddings()

@@ -86,14 +86,34 @@ def conv3x3(x, w9, *, bias=None, rowgroup=None, residual=None, out_dtype=BF16, f
     return out
 
 
-def conv3x3_s2(x, w9, *, bias=None, force_bn=0):
-    """3x3 stride-2 pad-1 convolution on NHWC bf16 (Downsample2D): (B,H,W,Cin) -> (B,H/2,W/2,Cout)."""
+def conv3x3_s2(x, w9, *, bias=None, force_bn=0, pad_lo=1):
+    """3x3 stride-2 convolution on NHWC bf16 (Downsample2D): (B,H,W,Cin) -> (B,H/2,W/2,Cout).
+    pad_lo=1: pad 1 on every side; pad_lo=0: one zero row / column on the bottom and right only (diffusers
+    Downsample2D(padding=0), the VAE encoder)."""
     assert x.dtype == BF16 and w9.dtype == BF16 and x.is_contiguous() and w9.is_contiguous()
     Bn, H, W, Cin = x.shape
     Cout = w9.shape[1]
     out = torch.empty((Bn, H // 2, W // 2, Cout), device=x.device, dtype=BF16)
-    _lib.call("e4t_conv3x3_s2_bf16", ptr(x), ptr(w9), ptr(out), c_int(Bn), c_int(H), c_int(W), c_int(Cin), c_int(Cout),
-              ptr(bias), c_int(force_bn), stream())
+    if pad_lo == 1:
+        _lib.call("e4t_conv3x3_s2_bf16", ptr(x), ptr(w9), ptr(out), c_int(Bn), c_int(H), c_int(W), c_int(Cin),
+                  c_int(Cout), ptr(bias), c_int(force_bn), stream())
+    else:
+        _lib.call("e4t_conv3x3_s2p_bf16", ptr(x), ptr(w9), ptr(out), c_int(Bn), c_int(H), c_int(W), c_int(Cin),
+                  c_int(Cout), c_int(pad_lo), ptr(bias), c_int(force_bn), stream())
+    return out
+
+
+def softmax_rows(x, out=None):
+    """bf16 softmax over the last dim of fp32 scores x (.., n); rows may be strided (last dim contiguous)."""
+    assert x.dtype == F32 and x.stride(-1) == 1
+    n = x.shape[-1]
+    x2 = x if x.dim() == 2 else x.reshape(-1, n)
+    if out is None:
+        out = torch.empty(x.shape, device=x.device, dtype=BF16)
+    assert out.dtype == BF16 and out.stride(-1) == 1 and out.shape == x.shape
+    o2 = out if out.dim() == 2 else out.view(-1, n)
+    _lib.call("e4t_softmax_rows", ptr(x2), ptr(o2), c_ll(x2.shape[0]), c_int(n), c_ll(x2.stride(0)), c_ll(o2.stride(0)),
+              stream())
     return out
 
 

@@ -39,7 +39,7 @@ int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, 
 /* 3x3 / stride 1 / pad 1 convolution as implicit GEMM (9 taps x Cin/64 K-chunks, halo by TMA zero fill).
  * Replaces nn.Conv2d inside diffusers ResnetBlock2D.conv1/conv2, Upsample2D.conv, Downsample2D.conv
  * (constructed at e4t/models/unet_2d_blocks.py:481-492,760-771,801-808,1732-1743,1773-1774) and their dgrad.
- * x [B][H][W][Cin] bf16 (Cin % 64 == 0, W | 128); w [9][Cout][Cin] bf16 (tap = ky*3+kx); out [B][H][W][Cout];
+ * x [B][H][W][Cin] bf16 (Cin % 64 == 0; output width W | 128, or W % 128 == 0 for wider rows); w [9][Cout][Cin] bf16 (tap = ky*3+kx); out [B][H][W][Cout];
  * bias fp32 [Cout]; rowgroup fp32 [B][Cout] (time-embedding projection added per image); residual bf16 like out. */
 int e4t_conv3x3_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout, int out_mode,
                      const float* bias, const float* rowgroup, const void* residual, int force_bn, void* stream);
@@ -49,6 +49,12 @@ int e4t_conv3x3_bf16(const void* x, const void* w, void* out, int B, int H, int 
  * out [B][H/2][W/2][Cout]. */
 int e4t_conv3x3_s2_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                         const float* bias, int force_bn, void* stream);
+/* 3x3 / stride 2 with pad_lo zero rows / columns on the top and left (1 = e4t_conv3x3_s2_bf16; 0 = diffusers
+ * Downsample2D(padding=0): `F.pad(x, (0, 1, 0, 1))` then an unpadded stride-2 conv, the VAE encoder's downsamplers built at
+ * e4t/models/unet_2d_blocks.py:937-1000 (DownEncoderBlock2D)).  Taps read x[2y + ky - pad_lo][2x + kx - pad_lo]; rows
+ * and columns outside the input are zero.  x [B][H][W][Cin] -> out [B][H/2][W/2][Cout]. */
+int e4t_conv3x3_s2p_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout, int pad_lo,
+                         const float* bias, int force_bn, void* stream);
 /* Weight gradient of the 3x3 / stride 1 / pad 1 convolution: dw9[tap][co][ci] += sum dy[b][y][x][co] * x[b][y+ky-1][x+kx-1][ci]
  * (fp32 atomic accumulation; implicit GEMM with 9 taps as the batch dimension, split-K over pixels).  Replaces autograd's
  * conv2d weight gradient when the base UNet is trainable (tuning_e4t.py:139-146; every requires_grad parameter under
@@ -84,6 +90,11 @@ int e4t_attn_bwd_fused_causal(const void* Q, const void* K, const void* V, const
                        long long ldq, long long q_bs, long long ldk, long long k_bs, long long ldv, long long v_bs,
                        long long ldo, long long o_bs, long long lddo, long long do_bs, long long lddq, long long dq_bs,
                        long long lddk, long long dk_bs, long long lddv, long long dv_bs, float scale, void* stream);
+
+/* Row softmax, fp32 scores in, bf16 probabilities out: y[r][:n] = softmax(x[r][:n]) (n % 4 == 0, n <= 16384, row strides
+ * ldx / ldy in elements).  Replaces `torch.softmax(attention_scores.float(), dim=-1).type(...)` of the VAE mid-block
+ * AttentionBlock (e4t/models/attention.py:165); the scores and P·V around it run on e4t_gemm_bf16. */
+int e4t_softmax_rows(const float* x, void* y, long long rows, int n, long long ldx, long long ldy, void* stream);
 
 /* Short-sequence attention (N, M <= 128, dh <= 64) with optional causal mask: the CLIP text tower's 77-token causal
  * self-attention (e4t/models/modeling_clip.py:45-51, HF CLIPAttention) and its backward.  Same layout as e4t_attn_fwd. */
