@@ -2,10 +2,13 @@
 text_model.embeddings.{token,position}_embedding, encoder.layers.{i}.{layer_norm1,self_attn.{q,k,v,out}_proj,
 layer_norm2,mlp.fc1,mlp.fc2}, final_layer_norm; causal mask; quick_gelu).
 
-Frozen weights, but dX must flow to the injected placeholder row (pretrain_e4t.py:630-634).  On CUDA the tower runs on
-the e4t_b200 kernels (round 2, SURVEY.md §8 f-3): LayerNorm kernel, one fused q|k|v wgmma GEMM with bias, the
-short-sequence causal attention kernel (77 tokens), out_proj / fc2 GEMMs with bias + residual epilogues, quick-GELU
-kernel; every Function returns dX.  CPU tensors (tokenizer-side utilities, tests of the module surface) take the plain
+Pre-training keeps the weights frozen, but dX must flow to the injected placeholder row (pretrain_e4t.py:630-634).  On
+CUDA the tower runs on the e4t_b200 kernels (round 2, SURVEY.md §8 f-3): LayerNorm kernel, one fused q|k|v wgmma GEMM
+with bias, the short-sequence causal attention kernel (77 tokens), out_proj / fc2 GEMMs with bias + residual epilogues,
+quick-GELU kernel; every Function returns dX.  Domain tuning with --train_text_encoder (tuning_e4t.py:127-146) also
+trains every text weight: each Function then returns its parameter gradients too (one dW GEMM for the fused q|k|v,
+the deterministic embedding-gradient kernel for the token table, a column sum for the position table); a frozen
+tower saves nothing for them and runs the same kernels as before.  CPU tensors (tokenizer-side utilities, tests of the module surface) take the plain
 torch path below — it is not used by any GPU step."""
 import json
 import os
@@ -31,6 +34,12 @@ def _f32(p):
 
 def _ln_k(norm, x):
     return FN.LayerNormFn.apply(x, _f32(norm.weight), _f32(norm.bias), norm.eps)
+
+
+def _linear_k(lin, x, residual):
+    """nn.Linear on the GEMM kernel; the fp32 master weight is passed for dW only when it is trained."""
+    w = lin.weight
+    return FN.LinearFn.apply(x, _bf16(w), _f32(lin.bias), residual, w if w.requires_grad else None)
 
 
 @dataclass
@@ -67,6 +76,21 @@ class _Embeddings(nn.Module):
         pos = self.position_embedding.weight[:n] if position_ids is None else self.position_embedding(position_ids)
         return inputs_embeds + pos
 
+    def trained(self):
+        return torch.is_grad_enabled() and (self.token_embedding.weight.requires_grad
+                                            or self.position_embedding.weight.requires_grad)
+
+    def forward_trained(self, input_ids=None, inputs_embeds=None):
+        """Embedding sum on the device when a table is trained (--train_text_encoder), as bf16 activations: the token
+        table takes its gradient from the embedding-gradient kernel, the position table from a column sum."""
+        tok, pos = self.token_embedding.weight, self.position_embedding.weight
+        if inputs_embeds is None:
+            inputs_embeds = FN.TokenEmbeddingFn.apply(input_ids, tok) if tok.requires_grad else tok.detach()[input_ids]
+        n = inputs_embeds.shape[1]
+        if pos.requires_grad:
+            return FN.PositionAddFn.apply(inputs_embeds.float(), pos[:n])
+        return FN.as_bf16(inputs_embeds + pos[:n])
+
 
 class _Attention(nn.Module):
     def __init__(self, cfg):
@@ -86,14 +110,14 @@ class _Attention(nn.Module):
 
     def forward_kernels(self, h, residual):
         D = h.shape[-1]
-        if torch.is_grad_enabled() and any(p.weight.requires_grad for p in (self.q_proj, self.k_proj, self.v_proj,
-                                                                             self.out_proj)):
-            raise NotImplementedError("--train_text_encoder is not supported: freeze the CLIP text tower "
-                                      "(text_encoder.requires_grad_(False), pretrain_e4t.py:262-263)")
         w, b = self._qkv()
-        qkv = FN.LinearFn.apply(h, w, b, None, None)
+        ps = (self.q_proj, self.k_proj, self.v_proj)
+        if torch.is_grad_enabled() and any(p.weight.requires_grad or p.bias.requires_grad for p in ps):
+            qkv = FN.QKVLinearFn.apply(h, w, b, *(p.weight for p in ps), *(p.bias for p in ps))
+        else:
+            qkv = FN.LinearFn.apply(h, w, b, None, None)
         o = FN.SmallAttentionFn.apply(qkv, self.heads, (D // self.heads) ** -0.5, True)   # causal (modeling_clip.py:45-47)
-        return FN.LinearFn.apply(o, _bf16(self.out_proj.weight), _f32(self.out_proj.bias), residual, None)
+        return _linear_k(self.out_proj, o, residual)
 
     def forward(self, x):
         B, N, D = x.shape
@@ -111,9 +135,9 @@ class _MLP(nn.Module):
         self.act = cfg.hidden_act
 
     def forward_kernels(self, h, residual):
-        h = FN.LinearFn.apply(h, _bf16(self.fc1.weight), _f32(self.fc1.bias), None, None)
+        h = _linear_k(self.fc1, h, None)
         h = FN.ActFn.apply(h, ops.ACT_QUICK_GELU if self.act == "quick_gelu" else ops.ACT_GELU)
-        return FN.LinearFn.apply(h, _bf16(self.fc2.weight), _f32(self.fc2.bias), residual, None)
+        return _linear_k(self.fc2, h, residual)
 
     def forward(self, x):
         h = self.fc1(x)
@@ -220,13 +244,19 @@ class CLIPTextModel(nn.Module):
             raise NotImplementedError("attention_mask is never passed on the E4T path")
         if input_ids is not None:
             input_ids = input_ids.view(-1, input_ids.shape[-1])
-        x = self.text_model.embeddings(input_ids=input_ids, inputs_embeds=inputs_embeds, position_ids=position_ids)
+        emb = self.text_model.embeddings
+        src = emb.token_embedding.weight if inputs_embeds is None else inputs_embeds
+        if src.is_cuda and position_ids is None and emb.trained():
+            out_dtype = torch.promote_types(src.dtype, emb.position_embedding.weight.dtype)
+            x = emb.forward_trained(input_ids=input_ids, inputs_embeds=inputs_embeds)
+        else:
+            x = emb(input_ids=input_ids, inputs_embeds=inputs_embeds, position_ids=position_ids)
+            out_dtype = x.dtype
         if x.is_cuda:
             N, D = x.shape[1], x.shape[2]
             dh = D // self.config.num_attention_heads
             if N > 128 or dh > 64 or dh % 8 != 0:
                 raise NotImplementedError(f"CLIP text tower on the e4t kernels needs N <= 128 and head dim <= 64 (got {N}, {dh})")
-            out_dtype = x.dtype
             x = _ln_k(self.text_model.final_layer_norm, self.text_model.encoder(FN.as_bf16(x))).to(out_dtype)
         else:
             x = self.text_model.final_layer_norm(self.text_model.encoder(x))

@@ -111,6 +111,14 @@ def save_e4t_unet(model, save_dir, save_all=False):
                    os.path.join(save_dir, "weight_offsets.pt"))
 
 
+def save_text_encoder(model, save_dir):
+    """text_encoder.pt = the text encoder's state dict (tuning_e4t.py:236-237, --train_text_encoder), as clones: under
+    the optimiser arena its parameters are views of one multi-GB storage.  inference.py:95-103 loads it with strict
+    missing / unexpected key checks."""
+    os.makedirs(save_dir, exist_ok=True)
+    torch.save(_detached(model.state_dict()), os.path.join(save_dir, "text_encoder.pt"))
+
+
 def save_config(args, save_dir, pretrained_args=None):
     """config.json as the training scripts write it (pretrain_e4t.py:230-234; nested `pretrained_args` when a run
     starts from an earlier E4T checkpoint, utils.py:76-89)."""

@@ -166,7 +166,7 @@ class PretrainStep:
     def __init__(self, unet, e4t_encoder, text_encoder, placeholder_token_id, class_token_id, lr=1.6e-5,
                  betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, domain_embed_scale=0.1, reg_lambda=0.01,
                  bos_id=49406, eos_id=49407, weight_dtype=torch.bfloat16, optimizer=True, tune_unet=False,
-                 max_grad_norm=None, vae=None):
+                 max_grad_norm=None, vae=None, train_text_encoder=False):
         self.unet, self.enc, self.text = unet, e4t_encoder, text_encoder
         # vae: an e4t AutoencoderKL; with it, a batch without "latents" is encoded on the device (pretrain_e4t.py:598-599)
         self.vae = vae
@@ -177,17 +177,24 @@ class PretrainStep:
         self.weight_dtype = weight_dtype
         dev = unet.device
         self.acp = ddpm_alphas_cumprod(device=dev)
-        self.text.requires_grad_(False)                                                  # pretrain_e4t.py:262-263
-        emb = self.text.get_input_embeddings()
-        with torch.no_grad():
-            self.class_embed = emb(torch.tensor([class_token_id], device=dev)).float()   # :561-564  (1,768)
-            ids = torch.tensor([[bos_id] + [eos_id] * 76], device=dev)
-            self.ehs_e4t = self.text(input_ids=ids)[0].to(weight_dtype)                  # :565-583  (1,77,768)
+        # train_text_encoder (tuning_e4t.py --train_text_encoder, :127-128,144-146): every text-encoder parameter is
+        # trained in fp32 next to the UNet; class_embed and ehs_e4t then follow the current weights at every step
+        self.train_text_encoder = bool(train_text_encoder)
+        if self.train_text_encoder and not tune_unet:
+            raise ValueError("train_text_encoder is a domain-tuning option (TuningStep)")
+        if self.train_text_encoder and any(p.dtype != torch.float32 for p in self.text.parameters()):
+            raise ValueError("train_text_encoder needs fp32 text-encoder weights (tuning_e4t.py --train_text_encoder)")
+        self.text.requires_grad_(self.train_text_encoder)                                # pretrain_e4t.py:262-263
+        self.class_ids = torch.tensor([class_token_id], device=dev)
+        self.ids_e4t = torch.tensor([[bos_id] + [eos_id] * 76], device=dev)
+        self.class_embed, self.ehs_e4t = self._text_constants()
         # tune_unet / max_grad_norm: the domain-tuning step (tuning_e4t.py:270-338): every UNet weight trainable,
         # global gradient-norm clipping over UNet + encoder parameters (:329-335)
         self.tune_unet, self.max_grad_norm = tune_unet, max_grad_norm
-        self.opt = FlatAdamW(trainable_parameters(unet, e4t_encoder, tune_unet), lr=lr, betas=betas,
-                             weight_decay=weight_decay, eps=eps) if optimizer else None
+        params = trainable_parameters(unet, e4t_encoder, tune_unet)
+        if self.train_text_encoder:
+            params += list(self.text.parameters())                                       # tuning_e4t.py:144-146
+        self.opt = FlatAdamW(params, lr=lr, betas=betas, weight_decay=weight_decay, eps=eps) if optimizer else None
         self._graph = None
         self.wo_bank = None
         self._wo_factor_exchange = False
@@ -221,6 +228,14 @@ class PretrainStep:
                     self.wo_bank.dp_group = True
                     self._wo_factor_exchange = True
 
+    def _text_constants(self):
+        """(class_embed (1,D) fp32, ehs_e4t (1,77,D)): the class token's table row and the encoding of the empty prompt
+        (pretrain_e4t.py:561-583; tuning_e4t.py:280-287 recomputes both from the current weights at every step)."""
+        with torch.no_grad():
+            class_embed = self.text.get_input_embeddings()(self.class_ids).float()
+            ehs_e4t = self.text(input_ids=self.ids_e4t)[0].to(self.weight_dtype)
+        return class_embed, ehs_e4t
+
     def placeholder_idxs(self, input_ids):
         """[ids.index(placeholder_id) for ids in input_ids] (pretrain_e4t.py:617) — exact integer bookkeeping."""
         return [row.index(self.placeholder_token_id) for row in input_ids.cpu().tolist()]
@@ -241,8 +256,12 @@ class PretrainStep:
         timesteps, input_ids = batch["timesteps"], batch["input_ids"]
         B = latents.shape[0]
         emb = self.text.get_input_embeddings()
-        with torch.no_grad():
-            inputs_embeds = emb(input_ids)                                               # :616
+        if self.train_text_encoder:
+            self.class_embed, self.ehs_e4t = self._text_constants()                      # tuning_e4t.py:280-287
+            inputs_embeds = FN.TokenEmbeddingFn.apply(input_ids, emb.weight)             # :297, with grad
+        else:
+            with torch.no_grad():
+                inputs_embeds = emb(input_ids)                                           # :616
         idxs = batch.get("placeholder_idxs")
         if idxs is None:
             idxs = self.placeholder_idxs(input_ids)                                      # :617
@@ -406,8 +425,11 @@ class PretrainStep:
 
 
 def TuningStep(unet, e4t_encoder, text_encoder, placeholder_token_id, class_token_id, lr=1.6e-5, reg_lambda=1e-4,
-               max_grad_norm=1.0, **kw):
+               max_grad_norm=1.0, train_text_encoder=False, **kw):
     """One optimisation step of tuning_e4t.py:270-338 (BASELINE.json configs[3]): the pre-training step with every UNet
-    weight and the encoder trainable, reg_lambda 1e-4 (tuning_e4t.py:31) and gradient-norm clipping at 1.0 (:38)."""
+    weight and the encoder trainable, reg_lambda 1e-4 (tuning_e4t.py:31) and gradient-norm clipping at 1.0 (:38).
+    train_text_encoder=True (--train_text_encoder, :48) also trains every fp32 text-encoder parameter: they follow the
+    UNet in the optimiser arena and in the clipped norm."""
     return PretrainStep(unet, e4t_encoder, text_encoder, placeholder_token_id, class_token_id, lr=lr,
-                        reg_lambda=reg_lambda, tune_unet=True, max_grad_norm=max_grad_norm, **kw)
+                        reg_lambda=reg_lambda, tune_unet=True, max_grad_norm=max_grad_norm,
+                        train_text_encoder=train_text_encoder, **kw)

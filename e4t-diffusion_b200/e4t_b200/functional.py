@@ -115,6 +115,84 @@ class LinearFn(torch.autograd.Function):
         return dx, None, db, (dy if ctx.has_res else None), dw
 
 
+class QKVLinearFn(torch.autograd.Function):
+    """LinearFn for a q|k|v projection whose three weights and biases are separate fp32 masters (the CLIP text tower's
+    q_proj / k_proj / v_proj): the forward is one GEMM with the row-concatenated bf16 operand `w` (3D, D) and fp32 bias.
+    Backward: dX, and — only for the masters that require grad — ONE dW GEMM (3D x D) and ONE column sum, whose row
+    blocks are returned as the three masters' gradients."""
+
+    @staticmethod
+    def forward(ctx, x, w, bias, wq, wk, wv, bq, bk, bv):
+        shp = x.shape
+        x2 = _c(x).view(-1, shp[-1])
+        y = ops.gemm(x2, w, bias=bias)
+        need_dw = any(ctx.needs_input_grad[3:6])
+        ctx.save_for_backward(w, x2 if need_dw else None)
+        ctx.shp = shp
+        return y.view(*shp[:-1], w.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        w, x2 = ctx.saved_tensors
+        N, K = w.shape
+        D = N // 3
+        dy2 = _c(dy).view(-1, N)
+        dx = ops.gemm(dy2, w, b_mn=True).view(ctx.shp) if ctx.needs_input_grad[0] else None
+        dws = dbs = (None, None, None)
+        if x2 is not None:
+            dw = torch.zeros((N, K), device=dy2.device, dtype=F32)
+            ops.gemm(dy2, x2, a_mn=True, b_mn=True, out=dw, accumulate=True, splits=_wgrad_splits(x2.shape[0], N, K))
+            dws = tuple(dw[i * D:(i + 1) * D] if ctx.needs_input_grad[3 + i] else None for i in range(3))
+        if any(ctx.needs_input_grad[6:9]):
+            db = ops.colsum_acc(dy2, torch.zeros(N, device=dy2.device, dtype=F32))
+            dbs = tuple(db[i * D:(i + 1) * D] if ctx.needs_input_grad[6 + i] else None for i in range(3))
+        return (dx, None, None) + dws + dbs
+
+
+class TokenEmbeddingFn(torch.autograd.Function):
+    """table[ids] (token-embedding lookup, tuning_e4t.py:297) with the table's gradient from the deterministic
+    e4t_embedding_grad kernel.  When an arena optimiser owns the table's .grad (FlatAdamW), the kernel adds into that
+    view directly instead of returning a dense (V, D) gradient for autograd to add."""
+
+    @staticmethod
+    def forward(ctx, ids, table):
+        ctx.save_for_backward(ids)
+        ctx.table = table
+        return table.detach()[ids]
+
+    @staticmethod
+    def backward(ctx, dy):
+        (ids,) = ctx.saved_tensors
+        table = ctx.table
+        if not ctx.needs_input_grad[1]:
+            return None, None
+        if DIRECT_GRAD_WRITE and getattr(table, "_e4t_arena", False) and table.grad is not None:
+            ops.embedding_grad(ids, dy, table.grad)
+            return None, None
+        return None, ops.embedding_grad(ids, dy, torch.zeros(table.shape, device=dy.device, dtype=F32))
+
+
+class PositionAddFn(torch.autograd.Function):
+    """bf16(x + pos) for token embeddings x (B, N, D) and the position table rows pos (N, D), both fp32 — the CLIP text
+    tower's embedding sum rounded to its bf16 activations.  Backward: dX = dY, dpos = sum over the batch of dY as one
+    column sum of dY viewed as (B, N*D)."""
+
+    @staticmethod
+    def forward(ctx, x, pos):
+        ctx.shp = x.shape
+        return (x + pos).to(BF16)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dy = _c(dy)
+        B, N, D = ctx.shp
+        dx = dy.float() if ctx.needs_input_grad[0] else None
+        dpos = None
+        if ctx.needs_input_grad[1]:
+            dpos = ops.colsum_acc(dy.view(B, N * D), torch.zeros(N * D, device=dy.device, dtype=F32)).view(N, D)
+        return dx, dpos
+
+
 class BatchedLinearFn(torch.autograd.Function):
     """Y[i] = X[i] @ W[i]ᵀ for a stack of independent linears (E4TEncoder's 129 first_linears, encoder.py:159-162, as ONE
     batched wgmma GEMM instead of 129 launches).  x (n,B,K) bf16; w16 (n,N,K) bf16 operand copy of the stacked fp32

@@ -397,6 +397,19 @@ def colsum_acc(x2, out, rows_per_group=0):
     return out
 
 
+def embedding_grad(ids, dx, out):
+    """out[ids[p]] += dx[p] for every position p (out fp32 (V, D), e.g. a token table's .grad; dx fp32 or bf16 (..., D)
+    over ids' positions).  Deterministic: each table row is summed by one block in position order."""
+    D = out.shape[1]
+    ids = ids.reshape(-1)
+    dx = dx.contiguous().view(-1, D)
+    assert ids.dtype == torch.int64 and dx.shape[0] == ids.numel()
+    assert dx.dtype in (F32, BF16) and out.dtype == F32 and out.dim() == 2 and out.is_contiguous()
+    _lib.call("e4t_embedding_grad", ptr(ids), ptr(dx), c_int(int(dx.dtype == F32)), ptr(out), c_ll(ids.numel()),
+              c_int(D), c_ll(out.shape[0]), stream())
+    return out
+
+
 def attn_small_fwd(q, k, v, heads, scale=None, causal=False):
     """Short-sequence attention (N, M <= 128, dh <= 64) with optional causal mask; same layout as attn_fwd."""
     assert q.dtype == BF16 and k.dtype == BF16 and v.dtype == BF16

@@ -139,6 +139,12 @@ int e4t_act_bwd(const void* x, const void* dy, void* dx, long long n, int mode, 
 /* out[g][n] += sum over the rows of group g (rows_per_group consecutive rows; <= 0: one group) of X[m][n]: bias gradients
  * and the per-image time-embedding-row gradient of ResnetBlock2D. */
 int e4t_colsum_acc(const void* X, float* out, long long M, int N, long long ld, long long rows_per_group, void* stream);
+/* Token-embedding gradient (CLIP text tower under --train_text_encoder, tuning_e4t.py:297): dE[ids[p]][:] += dX[p][:]
+ * for p < P <= 12288; ids int64, dX (P, D) contiguous, fp32 (dx_f32 = 1) or bf16, dE fp32 (V, D).  Deterministic (each
+ * table row is summed by one block in position order, no atomics) and free of host synchronisation; ids outside
+ * [0, V) are skipped. */
+int e4t_embedding_grad(const long long* ids, const void* dX, int dx_f32, float* dE, long long P, int D, long long V,
+                       void* stream);
 /* Weight gradients of the UNet's two narrow 3x3 convolutions (conv_in 4->C, unet_2d_condition.py:481; conv_out C->4, :557):
  * acc[w][n][tap] += sum wide[b][y][x][w] * narrow[b][n][y+sgn*(ky-1)][x+sgn*(kx-1)]; wide bf16 NHWC, narrow fp32 NCHW (<= 4 ch). */
 int e4t_narrow_conv_wgrad(const void* wide, const float* narrow, float* acc, int B, int H, int W, int Cw, int Cn, int sgn,
