@@ -53,6 +53,17 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 
+// ---- GroupNorm statistics ----------------------------------------------------------------------
+// fp32 [B][G][kGNStat] per (image, group) = (p, sum (x - p), sum (x - p)^2) over the group's n elements, where the
+// pivot p is the group's first element in that image.  Summing around p instead of 0 keeps E[x^2] - mean^2 from
+// cancelling when a group's mean is large against its spread (trained VAE / UNet activations).  Written by
+// e4t_groupnorm_fwd; every GroupNorm kernel turns it into (mean, rstd) here and nowhere else.
+static constexpr int kGNStat = 3;
+__device__ __forceinline__ float2 gn_mean_rstd(const float* __restrict__ st, float inv_n, float eps) {
+  const float d = st[1] * inv_n;
+  return make_float2(st[0] + d, rsqrtf(fmaxf(st[2] * inv_n - d * d, 0.f) + eps));
+}
+
 // ---- mbarrier ------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");

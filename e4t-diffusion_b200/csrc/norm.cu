@@ -7,8 +7,8 @@
 #include <stdlib.h>
 
 // ---------------------------------------------------------------------------------------------
-// GroupNorm statistics: sums[b][g] = (sum x, sum x^2) over HW x (C/G) elements.   (sums pre-zeroed)
-// mode 0: plain stats of x.
+// GroupNorm statistics over HW x (C/G) elements per (image, group).   (sums pre-zeroed)
+// mode 0: the forward stats of x, laid out as gn_mean_rstd (common.cuh) reads them: [B][G][kGNStat].
 // mode 1: backward stats: (sum dxhat, sum dxhat*xhat) with dxhat = dy * act'(y0) * gamma.
 // ---------------------------------------------------------------------------------------------
 // Thread mapping (all four kernels): a thread owns ONE 8-channel vector column (16-byte loads, coalesced across
@@ -47,16 +47,16 @@ __device__ __forceinline__ void gn_thread_chan(GNChan* ch, const float* __restri
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int g = (c0 + j) / cpg;
-    const float s = stats[((long)b * G + g) * 2], ss = stats[((long)b * G + g) * 2 + 1];
-    const float mean = s * inv_n;
-    ch[j].mean = mean;
-    ch[j].rstd = rsqrtf(fmaxf(ss * inv_n - mean * mean, 0.f) + eps);
+    const float2 mr = gn_mean_rstd(stats + ((long)b * G + g) * kGNStat, inv_n, eps);
+    ch[j].mean = mr.x;
+    ch[j].rstd = mr.y;
     ch[j].gamma = gamma[c0 + j];
     ch[j].beta = beta[c0 + j];
   }
 }
 
-// sums[b][g] += (Σ a, Σ b) over this CTA's rows.  MODE 0: (x, x²).  MODE 1: (dxhat, dxhat·xhat).
+// MODE 0: sums[b][g] = (p, += Σ (x-p), += Σ (x-p)²) over this CTA's rows, p = x[b][0][g*cpg] (CTA 0 stores p).
+// MODE 1: sums[b][g] += (Σ dxhat, Σ dxhat·xhat), sums [B][G][2].
 template <int MODE>
 __global__ void __launch_bounds__(kGNMaxThreads)
 gn_stats_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dy, const float* __restrict__ fstats,
@@ -70,27 +70,34 @@ gn_stats_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dy, const f
   const int c0 = cv * 8;
   const int r0 = blockIdx.x * rows_per_cta;
   const int r1 = min(HW, r0 + rows_per_cta);
+  const int cpg = C / G;
+  const bf16* ximg = x + ((long)b * HW) * C;
   GNChan ch[8];
-  if (MODE == 1) gn_thread_chan(ch, fstats, gamma, beta, b, c0, C, G, 1.f / ((float)HW * (float)(C / G)), eps);
+  float piv[8];
+  if (MODE == 1) gn_thread_chan(ch, fstats, gamma, beta, b, c0, C, G, 1.f / ((float)HW * (float)cpg), eps);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) piv[j] = MODE == 0 ? __bfloat162float(ximg[(c0 + j) / cpg * cpg]) : 0.f;
   __syncthreads();
   float a0[8], a1[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) a0[j] = a1[j] = 0.f;
-  const bf16* xb = x + ((long)b * HW) * C + c0;
+  const bf16* xb = ximg + c0;
   const bf16* db = MODE == 1 ? dy + ((long)b * HW) * C + c0 : nullptr;
 #pragma unroll 4
   for (int r = r0 + rl; r < r1; r += rstep) {
     float xv[8];
-    unpack8(*reinterpret_cast<const uint4*>(xb + (long)r * C), xv);
+    // __ldg: one 16-byte load per row (ptxas split the plain uint4 dereference into four 4-byte loads)
+    unpack8(__ldg(reinterpret_cast<const uint4*>(xb + (long)r * C)), xv);
     if (MODE == 0) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        a0[j] += xv[j];
-        a1[j] += xv[j] * xv[j];
+        const float d = xv[j] - piv[j];
+        a0[j] += d;
+        a1[j] += d * d;
       }
     } else {
       float dv[8];
-      unpack8(*reinterpret_cast<const uint4*>(db + (long)r * C), dv);
+      unpack8(__ldg(reinterpret_cast<const uint4*>(db + (long)r * C)), dv);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float xh = (xv[j] - ch[j].mean) * ch[j].rstd;
@@ -104,7 +111,7 @@ gn_stats_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dy, const f
 #pragma unroll
   for (int j = 0; j < 8; ++j) schan[rl * C + c0 + j] = make_float2(a0[j], a1[j]);
   __syncthreads();
-  const int cpg = C / G;
+  constexpr int NS = MODE == 0 ? kGNStat : 2;
   for (int g = threadIdx.x; g < G; g += blockDim.x) {
     float s = 0.f, ss = 0.f;
     for (int q = 0; q < rstep; ++q)
@@ -113,8 +120,10 @@ gn_stats_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dy, const f
         s += p.x;
         ss += p.y;
       }
-    atomicAdd(&sums[((long)b * G + g) * 2], s);
-    atomicAdd(&sums[((long)b * G + g) * 2 + 1], ss);
+    float* sg = sums + ((long)b * G + g) * NS;
+    if (MODE == 0 && blockIdx.x == 0) sg[0] = __bfloat162float(ximg[g * cpg]);
+    atomicAdd(&sg[NS - 2], s);
+    atomicAdd(&sg[NS - 1], ss);
   }
 }
 
@@ -207,12 +216,12 @@ static int gn_block(int C) {
   return vpr * k;
 }
 
-// stats: fp32 [B][G][2] = (sum, sumsq); written by this call.
+// stats: fp32 [B][G][kGNStat] (common.cuh); written by this call.
 extern "C" int e4t_groupnorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats, int B,
                                  int HW, int C, int G, float eps, int act_silu, void* stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
   E4T_CHECK(C % G == 0 && C % 8 == 0 && C / 8 <= kGNMaxThreads, "e4t_groupnorm_fwd: unsupported C=%d G=%d", C, G);
-  E4T_CUDA(cudaMemsetAsync(stats, 0, (size_t)B * G * 2 * sizeof(float), st));
+  E4T_CUDA(cudaMemsetAsync(stats, 0, (size_t)B * G * kGNStat * sizeof(float), st));
   const int threads = gn_block(C);
   const int rows = gn_rows_per_cta(gn_stats_kernel<0>, threads, (size_t)C * sizeof(float2), C, B, HW);
   dim3 grid(cdiv(HW, rows), B);

@@ -143,7 +143,8 @@ extern "C" int e4t_colsum_acc(const void* X, float* out, long long M, int N, lon
 // Non-head blocks stop at their id's first occurrence, which in a batch of prompts is almost always in the first row.
 // The skewed case (the pad/EOS id fills most of every 77-token prompt: ~1,000 of 1,232 rows at B = 16) is one head per
 // column slice summing its run with 8 row loads in flight per thread.  The grid depends on P and D only, so the launch
-// can be captured in a CUDA graph.
+// can be captured in a CUDA graph.  A row's sum is plain fp32 in position order, so its rounding error grows with its
+// run: ~1e-6 of the row's own magnitude for the ~1,000-position pad row, which is ~30x the table's typical row.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float4 load_row4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ float4 load_row4(const bf16* p) {
@@ -229,15 +230,15 @@ extern "C" int e4t_embedding_grad(const long long* ids, const void* dX, int dx_f
 // dbeta[c] += sum_r dz[r][c], with xhat = (x - mean) * rstd and dz = dy (LayerNorm, GroupNorm) or dy * silu'(z),
 // z = xhat * gamma + beta (GroupNorm+SiLU).  Statistics:
 //   PERCOL = false (LayerNorm): stats fp32 [rows][2] = (mean, rstd) per row
-//   PERCOL = true  (GroupNorm): mean_c / rstd_c fp32 [rows / rows_per_group][C] per (image, channel)
+//   PERCOL = true  (GroupNorm): st0 = e4t_groupnorm_fwd's stats [rows / rows_per_group][G][kGNStat] (common.cuh)
 // ---------------------------------------------------------------------------------------------
 template <bool PERCOL>
 __global__ void __launch_bounds__(256) norm_param_grad_kernel(const bf16* __restrict__ X, const bf16* __restrict__ dY,
-                                                              const float* __restrict__ st0, const float* __restrict__ st1,
+                                                              const float* __restrict__ st0,
                                                               const float* __restrict__ gamma, const float* __restrict__ beta,
                                                               float* __restrict__ dgamma, float* __restrict__ dbeta,
                                                               long long rows, int C, int rows_per_block,
-                                                              long long rows_per_group, int silu) {
+                                                              long long rows_per_group, int G, float eps, int silu) {
   __shared__ float red[2][8][256 + 8];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int n0 = (blockIdx.x * 32 + tx) * 8;
@@ -246,23 +247,28 @@ __global__ void __launch_bounds__(256) norm_param_grad_kernel(const bf16* __rest
   if (m1 > rows) m1 = rows;
   float ag[8] = {0, 0, 0, 0, 0, 0, 0, 0}, ab[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   if (n0 < C) {
-    float gm[8], bt[8];
+    float gm[8], bt[8], mean[8], rstd[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       gm[j] = gamma[n0 + j];
       bt[j] = beta ? beta[n0 + j] : 0.f;
     }
+    const int cpg = PERCOL ? C / G : 1;
+    const float inv_n = PERCOL ? 1.f / ((float)rows_per_group * (float)cpg) : 0.f;
+    long long img = -1;
     for (long long m = m0 + ty; m < m1; m += 8) {
       const uint4 ux = *reinterpret_cast<const uint4*>(X + m * C + n0);
       const uint4 ud = *reinterpret_cast<const uint4*>(dY + m * C + n0);
       const uint32_t xs[4] = {ux.x, ux.y, ux.z, ux.w}, ds[4] = {ud.x, ud.y, ud.z, ud.w};
-      float mean[8], rstd[8];
       if (PERCOL) {
-        const long long g = m / rows_per_group;
+        if (m / rows_per_group != img) {   // the image changed: this thread's (mean, rstd) of its 8 channels
+          img = m / rows_per_group;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          mean[j] = st0[g * C + n0 + j];
-          rstd[j] = st1[g * C + n0 + j];
+          for (int j = 0; j < 8; ++j) {
+            const float2 mr = gn_mean_rstd(st0 + (img * G + (n0 + j) / cpg) * kGNStat, inv_n, eps);
+            mean[j] = mr.x;
+            rstd[j] = mr.y;
+          }
         }
       } else {
         const float mu = st0[m * 2], rs = st0[m * 2 + 1];
@@ -326,22 +332,22 @@ extern "C" int e4t_layernorm_param_grad(const void* x, const void* dy, const flo
   int gx, rpb; long long gy;
   norm_grid(rows, C, gx, gy, rpb);
   norm_param_grad_kernel<false><<<dim3(gx, (unsigned)gy), 256, 0, (cudaStream_t)stream_>>>(
-      (const bf16*)x, (const bf16*)dy, stats, nullptr, gamma, nullptr, dgamma, dbeta, rows, C, rpb, 1, 0);
+      (const bf16*)x, (const bf16*)dy, stats, gamma, nullptr, dgamma, dbeta, rows, C, rpb, 1, 1, 0.f, 0);
   E4T_COUNT_LAUNCH();
   E4T_LAUNCH_CHECK();
   return 0;
 }
-// GroupNorm(+SiLU): x, dy bf16 [B*HW][C]; mean_c / rstd_c fp32 [B][C] (group statistics expanded per channel).
-extern "C" int e4t_groupnorm_param_grad(const void* x, const void* dy, const float* mean_c, const float* rstd_c,
-                                        const float* gamma, const float* beta, float* dgamma, float* dbeta, int B, int HW,
-                                        int C, int act_silu, void* stream_) {
-  E4T_CHECK(C % 8 == 0, "e4t_groupnorm_param_grad: C %% 8 != 0");
+// GroupNorm(+SiLU): x, dy bf16 [B*HW][C]; stats fp32 [B][G][kGNStat] as written by e4t_groupnorm_fwd.
+extern "C" int e4t_groupnorm_param_grad(const void* x, const void* dy, const float* stats, const float* gamma,
+                                        const float* beta, float* dgamma, float* dbeta, int B, int HW, int C, int G,
+                                        float eps, int act_silu, void* stream_) {
+  E4T_CHECK(C % 8 == 0 && C % G == 0, "e4t_groupnorm_param_grad: unsupported C=%d G=%d", C, G);
   const long long rows = (long long)B * HW;
   if (rows <= 0) return 0;
   int gx, rpb; long long gy;
   norm_grid(rows, C, gx, gy, rpb);
   norm_param_grad_kernel<true><<<dim3(gx, (unsigned)gy), 256, 0, (cudaStream_t)stream_>>>(
-      (const bf16*)x, (const bf16*)dy, mean_c, rstd_c, gamma, beta, dgamma, dbeta, rows, C, rpb, HW, act_silu);
+      (const bf16*)x, (const bf16*)dy, stats, gamma, beta, dgamma, dbeta, rows, C, rpb, HW, G, eps, act_silu);
   E4T_COUNT_LAUNCH();
   E4T_LAUNCH_CHECK();
   return 0;

@@ -121,12 +121,14 @@ def softmax_rows(x, out=None):
 # normalisation
 # ----------------------------------------------------------------------------------------------
 def groupnorm_fwd(x, gamma, beta, groups, eps, silu):
-    """x: (B,HW,C) or (B,H,W,C) bf16 NHWC.  Returns (y, stats[B,G,2] = (sum, sumsq))."""
+    """x: (B,HW,C) or (B,H,W,C) bf16 NHWC.  Returns (y, stats): stats fp32 [B,G,3] = (p, sum(x - p), sum((x - p)^2))
+    per (image, group) around the pivot p = the group's first element, the form groupnorm_bwd and
+    groupnorm_param_grad take (csrc/common.cuh, gn_mean_rstd, turns it into (mean, rstd))."""
     assert x.dtype == BF16 and x.is_contiguous()
     Bn, C = x.shape[0], x.shape[-1]
     HW = x.numel() // (Bn * C)
     y = torch.empty_like(x)
-    stats = torch.empty((Bn, groups, 2), device=x.device, dtype=F32)
+    stats = torch.empty((Bn, groups, 3), device=x.device, dtype=F32)
     _lib.call("e4t_groupnorm_fwd", ptr(x), ptr(gamma), ptr(beta), ptr(y), ptr(stats), c_int(Bn), c_int(HW), c_int(C),
               c_int(groups), c_float(eps), c_int(int(silu)), stream())
     return y, stats
@@ -455,19 +457,15 @@ def layernorm_param_grad(x, dy, stats, gamma):
 
 
 def groupnorm_param_grad(x, dy, stats, gamma, beta, groups, eps, silu):
-    """(dgamma, dbeta) fp32 of GroupNorm(+SiLU); stats = the forward's (sum, sum of squares) per (image, group)."""
+    """(dgamma, dbeta) fp32 of GroupNorm(+SiLU); stats = groupnorm_fwd's stats of x."""
+    assert x.is_contiguous() and dy.is_contiguous() and stats.is_contiguous()
     Bn, C = x.shape[0], x.shape[-1]
     HW = x.numel() // (Bn * C)
-    n = float(HW * (C // groups))
-    mean = stats[..., 0] / n
-    var = (stats[..., 1] / n - mean * mean).clamp_min(0.0)
-    rstd = torch.rsqrt(var + eps)
-    mean_c = mean.repeat_interleave(C // groups, dim=1).contiguous()
-    rstd_c = rstd.repeat_interleave(C // groups, dim=1).contiguous()
+    assert stats.shape == (Bn, groups, 3)
     dg = torch.zeros(C, device=x.device, dtype=F32)
     db = torch.zeros(C, device=x.device, dtype=F32)
-    _lib.call("e4t_groupnorm_param_grad", ptr(x), ptr(dy), ptr(mean_c), ptr(rstd_c), ptr(gamma), ptr(beta), ptr(dg),
-              ptr(db), c_int(Bn), c_int(HW), c_int(C), c_int(int(silu)), stream())
+    _lib.call("e4t_groupnorm_param_grad", ptr(x), ptr(dy), ptr(stats), ptr(gamma), ptr(beta), ptr(dg), ptr(db),
+              c_int(Bn), c_int(HW), c_int(C), c_int(groups), c_float(eps), c_int(int(silu)), stream())
     return dg, db
 
 

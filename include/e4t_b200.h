@@ -110,7 +110,8 @@ int e4t_attn_small_bwd(const void* Q, const void* K, const void* V, const void* 
 /* ---- normalisation ------------------------------------------------------------------------------------------- */
 /* GroupNorm (+ optional fused SiLU).  Replaces nn.GroupNorm + F.silu in diffusers ResnetBlock2D, Transformer2DModel
  * .norm (transformer_2d.py:149,253) and conv_norm_out/conv_act (unet_2d_condition.py:554-556).
- * x,y [B][HW][C] bf16; stats fp32 [B][G][2] = (sum, sum of squares), written by fwd and consumed by bwd. */
+ * x,y [B][HW][C] bf16; stats fp32 [B][G][3] = (p, sum (x - p), sum (x - p)^2) with the pivot p = x[b][0][g*C/G] (the
+ * group's first element), written by fwd and consumed by bwd and param_grad. */
 int e4t_groupnorm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* stats, int B, int HW,
                       int C, int G, float eps, int act_silu, void* stream);
 int e4t_groupnorm_bwd(const void* x, const void* dy, const float* gamma, const float* beta, const float* stats,
@@ -124,11 +125,11 @@ int e4t_layernorm_bwd(const void* x, const void* dy, const float* gamma, const f
 
 /* Affine-parameter gradients (accumulating into fp32 dgamma / dbeta), needed when the norms are trainable
  * (tuning_e4t.py:139-146, --unfreeze_clip_vision).  LayerNorm: stats as written by e4t_layernorm_fwd.  GroupNorm(+SiLU):
- * mean_c / rstd_c fp32 [B][C] = the group statistics expanded per channel. */
+ * stats as written by e4t_groupnorm_fwd. */
 int e4t_layernorm_param_grad(const void* x, const void* dy, const float* stats, const float* gamma, float* dgamma,
                              float* dbeta, long long rows, int C, void* stream);
-int e4t_groupnorm_param_grad(const void* x, const void* dy, const float* mean_c, const float* rstd_c, const float* gamma,
-                             const float* beta, float* dgamma, float* dbeta, int B, int HW, int C, int act_silu,
+int e4t_groupnorm_param_grad(const void* x, const void* dy, const float* stats, const float* gamma, const float* beta,
+                             float* dgamma, float* dbeta, int B, int HW, int C, int G, float eps, int act_silu,
                              void* stream);
 
 /* ---- elementwise --------------------------------------------------------------------------------------------- */

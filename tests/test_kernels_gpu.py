@@ -58,6 +58,73 @@ def test_layernorm(rows, C):
     assert _rel(dx, xr.grad) < 4e-3
 
 
+# Inputs bf16(mu + sd * randn) with a large mean against the spread, as trained checkpoints produce (SD's VAE decoder is
+# known for them): mu / sd = 0, 16, 64, 256, and nearly constant groups (sd 0.01 around 3).  Past ~256 bf16 itself
+# erases the spread (its spacing at 256 is 2).  The reference is fp64 on the same bf16 values.
+_OFFSETS = [(0.0, 1.0), (16.0, 1.0), (64.0, 1.0), (256.0, 1.0), (3.0, 0.01)]
+_OFFSET_IDS = ["mu0", "mu16", "mu64", "mu256", "const3"]
+
+
+def _ratio(x, dims):
+    """Largest |mean| / std of x's groups (reduced over dims), measured on the bf16 values."""
+    xd = x.double()
+    return (xd.mean(dims).abs() / xd.std(dims).clamp_min(1e-30)).max().item()
+
+
+@pytest.mark.parametrize("mu,sd", _OFFSETS, ids=_OFFSET_IDS)
+@pytest.mark.parametrize("B,HW,C", [(2, 4096, 320), (1, 512 * 512, 128), (2, 64, 1280)],
+                         ids=["unet_level0", "vae_512", "c1280_8x8"])
+@pytest.mark.parametrize("silu", [False, True])
+def test_groupnorm_offset(B, HW, C, silu, mu, sd):
+    """GroupNorm(+SiLU) forward, dx and the affine gradients against fp64 torch when a group's mean is large against
+    its spread: the statistics must not cancel (E[x^2] - mean^2 in fp32 loses all digits at mu / sd ~ 256)."""
+    from e4t_b200 import ops
+    g = torch.Generator(device="cuda").manual_seed(C + HW + int(mu))
+    x = _mk((B, HW, C), g, sd, mu)
+    gamma = torch.randn(C, generator=g, device="cuda") * 0.3 + 1
+    beta = torch.randn(C, generator=g, device="cuda") * 0.2
+    dy = _mk((B, HW, C), g)
+    ratio = _ratio(x.view(B, HW, 32, C // 32), (1, 3))
+    xr = x.double().permute(0, 2, 1).requires_grad_(True)
+    gr, br = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
+    yr = F.group_norm(xr, 32, gr, br, 1e-5)
+    if silu:
+        yr = F.silu(yr)
+    yr.backward(dy.double().permute(0, 2, 1))
+    y, stats = ops.groupnorm_fwd(x, gamma, beta, 32, 1e-5, silu)
+    dx = ops.groupnorm_bwd(x, dy, gamma, beta, stats, 32, 1e-5, silu)
+    dg, db = ops.groupnorm_param_grad(x, dy, stats, gamma, beta, 32, 1e-5, silu)
+    errs = dict(y=_rel(y.permute(0, 2, 1), yr), dx=_rel(dx.permute(0, 2, 1), xr.grad), dgamma=_rel(dg, gr.grad),
+                dbeta=_rel(db, br.grad))
+    print(f"[groupnorm {B}x{HW}x{C} silu={silu} mu/sd={ratio:.1f}] " + " ".join(f"{k} {v:.2e}" for k, v in errs.items()))
+    for k, v in errs.items():
+        assert v < 4e-3, (k, v, ratio)
+
+
+@pytest.mark.parametrize("mu,sd", _OFFSETS, ids=_OFFSET_IDS)
+@pytest.mark.parametrize("rows,C", [(2 * 4096, 320), (128, 1280), (300, 1024)])
+def test_layernorm_offset(rows, C, mu, sd):
+    """LayerNorm forward, dx and the affine gradients against fp64 torch with large row means (two-pass statistics)."""
+    from e4t_b200 import ops
+    g = torch.Generator(device="cuda").manual_seed(C + rows + int(mu))
+    x = _mk((rows, C), g, sd, mu)
+    gamma = torch.randn(C, generator=g, device="cuda") * 0.3 + 1
+    beta = torch.randn(C, generator=g, device="cuda") * 0.2
+    dy = _mk((rows, C), g)
+    ratio = _ratio(x, (1,))
+    xr = x.double().requires_grad_(True)
+    gr, br = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
+    F.layer_norm(xr, (C,), gr, br, 1e-5).backward(dy.double())
+    y, stats = ops.layernorm_fwd(x, gamma, beta, 1e-5)
+    dx = ops.layernorm_bwd(x, dy, gamma, stats, 1e-5)
+    dg, db = ops.layernorm_param_grad(x, dy, stats, gamma)
+    errs = dict(y=_rel(y, F.layer_norm(x.double(), (C,), gamma.double(), beta.double(), 1e-5)), dx=_rel(dx, xr.grad),
+                dgamma=_rel(dg, gr.grad), dbeta=_rel(db, br.grad))
+    print(f"[layernorm {rows}x{C} mu/sd={ratio:.1f}] " + " ".join(f"{k} {v:.2e}" for k, v in errs.items()))
+    for k, v in errs.items():
+        assert v < 4e-3, (k, v, ratio)
+
+
 def test_geglu_and_resample():
     from e4t_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(3)
