@@ -72,3 +72,45 @@ int e4t_tmap_encode(CUtensorMap* map, const void* gptr, int rank, const uint64_t
   }
   return 0;
 }
+
+typedef CUresult (*PFN_encodeIm2col)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                     const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t,
+                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+static PFN_encodeIm2col g_encode_im2col = nullptr;
+
+int e4t_tmap_encode_im2col(CUtensorMap* map, const void* gptr, const uint64_t* dims, const uint64_t* strides_bytes,
+                           const int* lower, const int* upper, uint32_t channels, uint32_t pixels,
+                           const uint32_t* elem_strides) {
+  if (!g_encode_im2col) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &qres);
+    if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || !fn)
+      return e4t_set_error("cuTensorMapEncodeIm2col entry point unavailable (%s)", cudaGetErrorString(e));
+    g_encode_im2col = (PFN_encodeIm2col)fn;
+  }
+  static thread_local bool ctx_bound = false;  // as in e4t_tmap_encode
+  if (!ctx_bound) {
+    cudaFree(0);
+    ctx_bound = true;
+  }
+  cuuint64_t gdim[4], gstr[3];
+  cuuint32_t estr[4];
+  for (int i = 0; i < 4; ++i) {
+    gdim[i] = dims[i];
+    estr[i] = elem_strides[i];
+    if (i > 0) gstr[i - 1] = strides_bytes[i - 1];
+  }
+  CUresult r = g_encode_im2col(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(gptr), gdim, gstr, lower,
+                               upper, channels, pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return e4t_set_error(
+        "cuTensorMapEncodeIm2col failed (%d): dims=[%llu,%llu,%llu,%llu] corners=[%d,%d]..[%d,%d] pixels=%u "
+        "stride=%u ptr=%p",
+        (int)r, (unsigned long long)gdim[0], (unsigned long long)gdim[1], (unsigned long long)gdim[2],
+        (unsigned long long)gdim[3], lower[0], lower[1], upper[0], upper[1], pixels, estr[1], gptr);
+  return 0;
+}

@@ -41,6 +41,12 @@ int e4t_tmap_encode(CUtensorMap* map, const void* gptr, int rank, const uint64_t
                     const uint64_t* strides_bytes /* rank-1 entries, dims 1.. */,
                     const uint32_t* box, int elem_bytes /*2 = bf16*/, int swizzle_bytes = 128,
                     const uint32_t* elem_strides = nullptr /* traversal stride per dim (box is in global coordinates) */);
+// im2col-mode tensor map over an NHWC bf16 tensor, 128-byte swizzle: dims / strides as for e4t_tmap_encode (rank 4,
+// {C, W, H, N}); each load reads `pixels` pixels x `channels` channels.  lower / upper {W, H}: the bounding box a load
+// walks spans [lower, dim - 1 + upper] in W and H, stepped by elem_strides[1], [2].
+int e4t_tmap_encode_im2col(CUtensorMap* map, const void* gptr, const uint64_t* dims, const uint64_t* strides_bytes,
+                           const int* lower, const int* upper, uint32_t channels, uint32_t pixels,
+                           const uint32_t* elem_strides);
 
 static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 
@@ -135,6 +141,18 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* m, ui
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
       "[%2];" ::"r"(smem_u32(smem)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+// im2col mode (tensor map from e4t_tmap_encode_im2col, NHWC): (c, w, h, n) is the input position of the first pixel's
+// top-left tap; the load walks the map's pixelsPerColumn pixels in NHW order through its bounding box, across row and
+// image boundaries, and reads each one at (w + off_w, h + off_h), zero-filling reads outside the tensor.
+__device__ __forceinline__ void tma_load_im2col_4d(void* smem, const CUtensorMap* m, uint64_t* bar, int c, int w,
+                                                   int h, int n, int off_w, int off_h) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
+      "%6}], [%2], {%7, %8};" ::"r"(smem_u32(smem)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n),
+      "h"((uint16_t)off_w), "h"((uint16_t)off_h)
       : "memory");
 }
 

@@ -170,7 +170,10 @@ __device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUten
   }
 }
 
-template <int BN, int AMN, int BMN>
+// IM2COL: the implicit convolution's pixel operand (conv = 1: A, conv = 2: B) is an im2col-mode tensor map instead
+// of a tiled 4-D box.  A template argument rather than a GemmArgs field, so the kernels every other call runs compile
+// to exactly the code they had without it.
+template <int BN, int AMN, int BMN, bool IM2COL>
 __global__ void __launch_bounds__(kThreads, 1)
 e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                 const __grid_constant__ CUtensorMap mapO, const GemmArgs g) {
@@ -211,12 +214,14 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
       const int m0 = m_t * kBM, n0 = n_t * BN;
       const int kc0 = sp * g.kper;
       const int kc1 = min(g.kchunks, kc0 + g.kper);
+      // (image, row, column) of the tile's first output pixel; with the tiled box the column is non-zero only for
+      // rows wider than a tile (W > 128: a tile is 128 pixels of one row), with im2col a tile starts anywhere
       int cb0 = 0, ch0 = 0, cw0 = 0;
       if (g.conv == 1) {
         const int img = g.H * g.W;
         cb0 = m0 / img;
         ch0 = (m0 % img) / g.W;
-        cw0 = m0 % g.W;  // non-zero only for rows wider than a tile (W > 128: a tile is 128 pixels of one row)
+        cw0 = m0 % g.W;
       }
       for (int kc = kc0; kc < kc1; ++kc) {
         mbar_wait(&empty_bar[s], ph ^ 1u);
@@ -227,18 +232,28 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
           // 3x3 weight gradient: dW[tap][co][ci] = sum_p dY[p][co] * X[p + tap][ci].  A = dY (MN-major, 64 pixels of
           // K per chunk), B = the tap-shifted input pixels (MN-major; same 4-D box + out-of-bounds zero fill as the
           // forward's A operand, 64 pixels x 64 channels per N chunk); batch index = tap
+          // (im2col: 64 consecutive pixels from any first pixel, across rows and images; past the last pixel both
+          // dY and X read as zero)
           const int tap = bz, dy = tap / 3, dx = tap % 3;
           const int p0 = kc * kBK, img = g.H * g.W;
           const int b0 = p0 / img, h0 = (p0 % img) / g.W;
           tma_load_3d(sA, &mapA, &full_bar[s], m0, p0, 0);
           tma_load_3d(sA + 8192, &mapA, &full_bar[s], m0 + 64, p0, 0);
-          for (int i = 0; i < BN / 64; ++i)
-            tma_load_4d(sB + i * 8192, &mapB, &full_bar[s], n0 + 64 * i, dx - 1, h0 + dy - 1, b0);
+          for (int i = 0; i < BN / 64; ++i) {
+            if constexpr (IM2COL)
+              tma_load_im2col_4d(sB + i * 8192, &mapB, &full_bar[s], n0 + 64 * i, p0 % g.W - 1, h0 - 1, b0, dx, dy);
+            else
+              tma_load_4d(sB + i * 8192, &mapB, &full_bar[s], n0 + 64 * i, dx - 1, h0 + dy - 1, b0);
+          }
         } else if (g.conv) {
           const int tap = kc / g.cin_chunks, cc = kc % g.cin_chunks;
           const int dy = tap / 3, dx = tap % 3;
-          tma_load_4d(sA, &mapA, &full_bar[s], cc * kBK, g.cstride * cw0 + dx - g.cpad, g.cstride * ch0 + dy - g.cpad,
-                      cb0);
+          if constexpr (IM2COL)
+            tma_load_im2col_4d(sA, &mapA, &full_bar[s], cc * kBK, g.cstride * cw0 - g.cpad, g.cstride * ch0 - g.cpad,
+                               cb0, dx, dy);
+          else
+            tma_load_4d(sA, &mapA, &full_bar[s], cc * kBK, g.cstride * cw0 + dx - g.cpad,
+                        g.cstride * ch0 + dy - g.cpad, cb0);
           tma_load_2d(sB, &mapB, &full_bar[s], cc * kBK, tap * g.cout + n0);
         } else {
           const int ab = g.a_batched ? bz : 0, bb = g.b_batched ? bz : 0;
@@ -388,7 +403,7 @@ static int auto_splits(int N, long m_tiles_x_batch, bool b_mn, int kchunks) {
   return best;
 }
 
-template <int BN, int AMN, int BMN>
+template <int BN, int AMN, int BMN, bool IM2COL>
 static int launch_gemm_t(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, GemmArgs& g, int grid,
                          cudaStream_t stream) {
   constexpr int stage_bytes = kATileBytes + BN * kBK * 2;
@@ -400,36 +415,38 @@ static int launch_gemm_t(const CUtensorMap& mA, const CUtensorMap& mB, const CUt
   const size_t smem = (size_t)stages * stage_bytes + 2 * kStgBytes<BN> + 2 * stages * sizeof(uint64_t) + 1024;
   static bool attr_set = false;
   if (!attr_set) {
-    E4T_CUDA(cudaFuncSetAttribute(e4t_gemm_kernel<BN, AMN, BMN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    E4T_CUDA(cudaFuncSetAttribute(e4t_gemm_kernel<BN, AMN, BMN, IM2COL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   227 * 1024));
     attr_set = true;
   }
-  e4t_gemm_kernel<BN, AMN, BMN><<<grid, kThreads, smem, stream>>>(mA, mB, mO, g);
+  e4t_gemm_kernel<BN, AMN, BMN, IM2COL><<<grid, kThreads, smem, stream>>>(mA, mB, mO, g);
   E4T_COUNT_LAUNCH();
   E4T_LAUNCH_CHECK();
   return 0;
 }
 
-template <int AMN, int BMN>
+template <int AMN, int BMN, bool IM2COL>
 static int launch_gemm_bn(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, GemmArgs& g, int grid,
                           cudaStream_t stream) {
   switch (g.BN) {
-    case 64: return launch_gemm_t<64, AMN, BMN>(mA, mB, mO, g, grid, stream);
-    case 128: return launch_gemm_t<128, AMN, BMN>(mA, mB, mO, g, grid, stream);
-    case 192: return launch_gemm_t<192, AMN, BMN>(mA, mB, mO, g, grid, stream);
-    case 256: return launch_gemm_t<256, AMN, BMN>(mA, mB, mO, g, grid, stream);
+    case 64: return launch_gemm_t<64, AMN, BMN, IM2COL>(mA, mB, mO, g, grid, stream);
+    case 128: return launch_gemm_t<128, AMN, BMN, IM2COL>(mA, mB, mO, g, grid, stream);
+    case 192: return launch_gemm_t<192, AMN, BMN, IM2COL>(mA, mB, mO, g, grid, stream);
+    case 256: return launch_gemm_t<256, AMN, BMN, IM2COL>(mA, mB, mO, g, grid, stream);
   }
-  if (!BMN) {
+  if constexpr (!BMN) {
     switch (g.BN) {
-      case 96: return launch_gemm_t<96, AMN, 0>(mA, mB, mO, g, grid, stream);
-      case 160: return launch_gemm_t<160, AMN, 0>(mA, mB, mO, g, grid, stream);
-      case 224: return launch_gemm_t<224, AMN, 0>(mA, mB, mO, g, grid, stream);
+      case 96: return launch_gemm_t<96, AMN, 0, IM2COL>(mA, mB, mO, g, grid, stream);
+      case 160: return launch_gemm_t<160, AMN, 0, IM2COL>(mA, mB, mO, g, grid, stream);
+      case 224: return launch_gemm_t<224, AMN, 0, IM2COL>(mA, mB, mO, g, grid, stream);
     }
   }
   return e4t_set_error("e4t_gemm_bf16: unsupported tile width BN=%d (b_mn=%d)", g.BN, BMN);
 }
 
-static int launch_gemm(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs& g, cudaStream_t stream) {
+// im2col: an implicit convolution whose pixel operand mA (forward) / mB (weight gradient) is an im2col-mode map.
+static int launch_gemm(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs& g, cudaStream_t stream,
+                       bool im2col = false) {
   const int esz = g.out_mode == 0 ? 2 : 4;
   g.pair_store = (g.ldo % 2) == 0 && (g.batch == 1 || (g.out_bstride % 2) == 0) && ((uintptr_t)g.out % (2 * esz)) == 0;
   // TMA addresses the output when its base is 16-byte aligned and its row pitch and batch stride are multiples of
@@ -451,9 +468,14 @@ static int launch_gemm(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs& g
   int grid = (int)(total < num_sms() ? total : num_sms());
   if (grid < 1) return 0;
   // the implicit convolutions load A K-major (wgrad: both operands MN-major, set in a_mn / b_mn)
+  if (im2col)
+    return g.a_mn ? launch_gemm_bn<1, 1, true>(mA, mB, mO, g, grid, stream)
+                  : launch_gemm_bn<0, 0, true>(mA, mB, mO, g, grid, stream);
   if (g.a_mn)
-    return g.b_mn ? launch_gemm_bn<1, 1>(mA, mB, mO, g, grid, stream) : launch_gemm_bn<1, 0>(mA, mB, mO, g, grid, stream);
-  return g.b_mn ? launch_gemm_bn<0, 1>(mA, mB, mO, g, grid, stream) : launch_gemm_bn<0, 0>(mA, mB, mO, g, grid, stream);
+    return g.b_mn ? launch_gemm_bn<1, 1, false>(mA, mB, mO, g, grid, stream)
+                  : launch_gemm_bn<1, 0, false>(mA, mB, mO, g, grid, stream);
+  return g.b_mn ? launch_gemm_bn<0, 1, false>(mA, mB, mO, g, grid, stream)
+                : launch_gemm_bn<0, 0, false>(mA, mB, mO, g, grid, stream);
 }
 
 extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, int batch, int a_mn,
@@ -530,34 +552,48 @@ extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int
 // stride 2 (diffusers Downsample2D): the A-operand tensor map walks the input with element strides (1,2,2,1), so the
 // tile of 128 OUTPUT pixels is gathered directly from every other input pixel — no stride-1 result is computed and
 // thrown away (round 1 did exactly that: 4x the FLOPs on the three downsampling convolutions).
-// Tiles: an output width W that divides 128 gives tiles of 128 / W whole rows (or whole images when H*W < 128); a
-// width W > 128 that is a multiple of 128 gives tiles of 128 consecutive pixels of one row, whose first column the
-// producer adds to the A-operand x coordinate.
+// Tiles, tiled box (im2col = 0): an output width W that divides 128 gives tiles of 128 / W whole rows (or whole images
+// when H*W < 128); a width W > 128 that is a multiple of 128 gives tiles of 128 consecutive pixels of one row, whose
+// first column the producer adds to the A-operand x coordinate.  conv_tiled_fits() is that domain.
+// im2col = 1: the A operand is an im2col-mode tensor map, so a tile is any 128 consecutive output pixels in NHW order,
+// across row and image boundaries, and every output size works.  Its bounding box starts at -pad_lo and ends on the
+// last tap-(0, 0) position, stride*(out - 1) - pad_lo, so each image yields exactly H x W output pixels; the tap's
+// (dx, dy) are the load's im2col offsets.  The shared-memory tile is byte-identical to the tiled box's (128 rows of 64
+// channels, SWIZZLE_128B), so the MMA warpgroups and the epilogue do not know which load filled it.
+static bool conv_tiled_fits(int H, int W) {
+  if (W > 128) return W % 128 == 0;
+  if (128 % W) return false;
+  return H * W >= 128 ? H % (128 / W) == 0 : 128 % (H * W) == 0;
+}
+
 static int conv3x3_impl(const void* x, const void* w, void* out, int B, int Hin, int Win, int Cin, int Cout, int stride,
                         int pad_lo, int out_mode, const float* bias, const float* rowgroup, const void* residual,
-                        int force_bn, cudaStream_t stream) {
+                        int force_bn, bool im2col, cudaStream_t stream) {
+  E4T_CHECK(B > 0 && Hin > 0 && Win > 0 && Cout > 0, "e4t_conv3x3: bad dims B=%d H=%d W=%d Cout=%d", B, Hin, Win, Cout);
   E4T_CHECK(Cin % 64 == 0, "e4t_conv3x3: Cin must be a multiple of 64 (got %d)", Cin);
   E4T_CHECK(stride == 1 || (stride == 2 && Hin % 2 == 0 && Win % 2 == 0), "e4t_conv3x3: bad stride/size");
   E4T_CHECK(pad_lo == 1 || (stride == 2 && pad_lo == 0), "e4t_conv3x3: bad padding %d for stride %d", pad_lo, stride);
   const int H = Hin / stride, W = Win / stride;
   const bool wide = W > 128;
-  E4T_CHECK((W <= 128 && (128 % W) == 0) || (wide && W % 128 == 0),
-            "e4t_conv3x3: output width must divide 128 or be a multiple of 128 (got %d)", W);
-  E4T_CHECK(out_mode == 0 || out_mode == 1, "e4t_conv3x3: bad out_mode");
   const int img = H * W;
-  int BH, BB;
-  if (wide) {
-    BB = 1;
-    BH = 1;
-  } else if (img >= 128) {
-    BB = 1;
-    BH = 128 / W;
-    E4T_CHECK(H % BH == 0, "e4t_conv3x3: H=%d not a multiple of tile height %d", H, BH);
-  } else {
-    E4T_CHECK(128 % img == 0, "e4t_conv3x3: H*W must divide 128");
-    BB = 128 / img;
-    BH = H;
+  int BH = 1, BB = 1;
+  if (!im2col) {
+    E4T_CHECK((W <= 128 && (128 % W) == 0) || (wide && W % 128 == 0),
+              "e4t_conv3x3: output width must divide 128 or be a multiple of 128 (got %d)", W);
+    if (wide) {
+      BB = 1;
+      BH = 1;
+    } else if (img >= 128) {
+      BB = 1;
+      BH = 128 / W;
+      E4T_CHECK(H % BH == 0, "e4t_conv3x3: H=%d not a multiple of tile height %d", H, BH);
+    } else {
+      E4T_CHECK(128 % img == 0, "e4t_conv3x3: H*W must divide 128");
+      BB = 128 / img;
+      BH = H;
+    }
   }
+  E4T_CHECK(out_mode == 0 || out_mode == 1, "e4t_conv3x3: bad out_mode");
   const int BW = wide ? 128 : W;
   GemmArgs g;
   memset(&g, 0, sizeof(g));
@@ -577,9 +613,15 @@ static int conv3x3_impl(const void* x, const void* w, void* out, int B, int Hin,
   {
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)Win, (uint64_t)Hin, (uint64_t)B};
     uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)Win * Cin * 2, (uint64_t)Hin * Win * Cin * 2};
-    uint32_t box[4] = {kBK, (uint32_t)(BW * stride), (uint32_t)(BH * stride), (uint32_t)BB};
     uint32_t es[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
-    if (int e = e4t_tmap_encode(&mA, x, 4, dims, str, box, 2, 128, stride == 1 ? nullptr : es)) return e;
+    if (im2col) {
+      const int lower[2] = {-pad_lo, -pad_lo};
+      const int upper[2] = {stride * (W - 1) - pad_lo - (Win - 1), stride * (H - 1) - pad_lo - (Hin - 1)};
+      if (int e = e4t_tmap_encode_im2col(&mA, x, dims, str, lower, upper, kBK, kBM, es)) return e;
+    } else {
+      uint32_t box[4] = {kBK, (uint32_t)(BW * stride), (uint32_t)(BH * stride), (uint32_t)BB};
+      if (int e = e4t_tmap_encode(&mA, x, 4, dims, str, box, 2, 128, stride == 1 ? nullptr : es)) return e;
+    }
   }
   {
     uint64_t dims[2] = {(uint64_t)Cin, (uint64_t)9 * Cout};
@@ -587,21 +629,30 @@ static int conv3x3_impl(const void* x, const void* w, void* out, int B, int Hin,
     uint32_t box[2] = {kBK, (uint32_t)g.BN};
     if (int e = e4t_tmap_encode(&mB, w, 2, dims, str, box, 2)) return e;
   }
-  return launch_gemm(mA, mB, g, stream);
+  return launch_gemm(mA, mB, g, stream, im2col);
 }
 
 extern "C" int e4t_conv3x3_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                                 int out_mode, const float* bias, const float* rowgroup, const void* residual,
                                 int force_bn, void* stream_) {
-  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 1, 1, out_mode, bias, rowgroup, residual, force_bn,
+  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 1, 1, out_mode, bias, rowgroup, residual, force_bn, false,
+                      (cudaStream_t)stream_);
+}
+
+// e4t_conv3x3_bf16 with the A operand in TMA im2col mode: any output size (tiles span rows and images).
+extern "C" int e4t_conv3x3_im2col_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
+                                       int out_mode, const float* bias, const float* rowgroup, const void* residual,
+                                       int force_bn, void* stream_) {
+  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 1, 1, out_mode, bias, rowgroup, residual, force_bn, true,
                       (cudaStream_t)stream_);
 }
 
 // 3x3 / stride 2 / pad 1 (diffusers Downsample2D.conv, e4t/models/unet_2d_blocks.py:801-808): x [B][H][W][Cin] ->
-// out [B][H/2][W/2][Cout].
+// out [B][H/2][W/2][Cout].  The tiled box where it covers the output size, im2col elsewhere.
 extern "C" int e4t_conv3x3_s2_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                                    const float* bias, int force_bn, void* stream_) {
-  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 2, 1, 0, bias, nullptr, nullptr, force_bn, (cudaStream_t)stream_);
+  return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 2, 1, 0, bias, nullptr, nullptr, force_bn,
+                      !conv_tiled_fits(H / 2, W / 2), (cudaStream_t)stream_);
 }
 
 // 3x3 / stride 2 with pad_lo zero rows / columns on the top and left: pad_lo = 1 is e4t_conv3x3_s2_bf16; pad_lo = 0 is
@@ -609,19 +660,21 @@ extern "C" int e4t_conv3x3_s2_bf16(const void* x, const void* w, void* out, int 
 extern "C" int e4t_conv3x3_s2p_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                                     int pad_lo, const float* bias, int force_bn, void* stream_) {
   return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 2, pad_lo, 0, bias, nullptr, nullptr, force_bn,
-                      (cudaStream_t)stream_);
+                      !conv_tiled_fits(H / 2, W / 2), (cudaStream_t)stream_);
 }
 
 // 3x3 / stride 1 / pad 1 weight gradient: dw9[tap][co][ci] += sum_{b,y,x} dy[b][y][x][co] * x[b][y+ky-1][x+kx-1][ci]
 // (tap = ky*3+kx; fp32 atomic accumulation, split-K over the pixels).  x NHWC bf16 [B][H][W][Cin], dy [B][H][W][Cout].
 // Replaces autograd's conv2d weight gradient behind every ResnetBlock2D / Upsample2D / Downsample2D conv when the base
-// UNet is trainable (tuning_e4t.py:139-146).  Cin, Cout % 64 == 0; W | 64; H*W % 64 == 0.
+// UNet is trainable (tuning_e4t.py:139-146).  Cin, Cout % 64 == 0.  Each K chunk is 64 consecutive pixels: a tiled
+// box of whole rows where W | 64 and H*W % 64 == 0, else an im2col-mode load (any image size; the last chunk's
+// pixels past B*H*W are zero in both operands).
 extern "C" int e4t_conv3x3_wgrad(const void* x, const void* dy, float* dw9, int B, int H, int W, int Cin, int Cout,
                                  void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   E4T_CHECK(Cin % 64 == 0 && Cout % 64 == 0, "e4t_conv3x3_wgrad: Cin, Cout must be multiples of 64 (%d, %d)", Cin, Cout);
-  E4T_CHECK(W <= 64 && (64 % W) == 0 && (H * W) % 64 == 0 && H % (64 / W) == 0,
-            "e4t_conv3x3_wgrad: unsupported image %dx%d (W | 64, H*W %% 64 == 0)", H, W);
+  E4T_CHECK(B > 0 && H > 0 && W > 0, "e4t_conv3x3_wgrad: bad image %dx%dx%d", B, H, W);
+  const bool im2col = !(W <= 64 && (64 % W) == 0 && (H * W) % 64 == 0 && H % (64 / W) == 0);
   const long long pixels = (long long)B * H * W;
   GemmArgs g;
   memset(&g, 0, sizeof(g));
@@ -629,7 +682,7 @@ extern "C" int e4t_conv3x3_wgrad(const void* x, const void* dy, float* dw9, int 
   g.a_mn = 1; g.b_mn = 1; g.a_batched = 0; g.b_batched = 1;
   g.conv = 2; g.H = H; g.W = W; g.cout = Cout; g.cstride = 1; g.cpad = 1;
   g.m_tiles = cdiv(Cout, kBM);
-  g.kchunks = (int)(pixels / kBK);
+  g.kchunks = cdiv(pixels, kBK);
   // enough K-splits to fill the machine about twice: tiles = 9 taps x m_tiles x n_tiles x splits
   const int base_tiles = 9 * g.m_tiles * cdiv(Cin, 256);
   int splits = cdiv(2 * num_sms(), base_tiles);
@@ -651,8 +704,14 @@ extern "C" int e4t_conv3x3_wgrad(const void* x, const void* dy, float* dw9, int 
   {
     uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
     uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-    uint32_t box[4] = {64, (uint32_t)W, (uint32_t)(64 / W), 1};
-    if (int e = e4t_tmap_encode(&mB, x, 4, dims, str, box, 2)) return e;
+    if (im2col) {
+      const int lower[2] = {-1, -1}, upper[2] = {-1, -1};   // the stride-1 pad-1 box: W x H tap-(0, 0) positions
+      const uint32_t es[4] = {1, 1, 1, 1};
+      if (int e = e4t_tmap_encode_im2col(&mB, x, dims, str, lower, upper, 64, kBK, es)) return e;
+    } else {
+      uint32_t box[4] = {64, (uint32_t)W, (uint32_t)(64 / W), 1};
+      if (int e = e4t_tmap_encode(&mB, x, 4, dims, str, box, 2)) return e;
+    }
   }
-  return launch_gemm(mA, mB, g, stream);
+  return launch_gemm(mA, mB, g, stream, im2col);
 }

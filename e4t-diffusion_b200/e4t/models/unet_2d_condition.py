@@ -159,6 +159,13 @@ class UNet2DConditionModel(ModelMixin, ConfigMixin):
         self.conv_act = nn.SiLU()
         self.conv_out = nn.Conv2d(block_out_channels[0], out_channels, kernel_size=3, padding=1)
 
+    @property
+    def latent_multiple(self) -> int:
+        """Latent heights and widths must be multiples of this: the overall down-sampling factor 2^(levels - 1) (8 for
+        SD-v1.4, i.e. images in multiples of 64 px), so every stride-2 convolution sees an even size and each up block
+        meets its skip connections at their size."""
+        return 2 ** (len(self.config.block_out_channels) - 1)
+
     # ---- processor plumbing (unet_2d_condition.py:291-341) ---------------------------------------
     @property
     def attn_processors(self) -> Dict[str, Any]:

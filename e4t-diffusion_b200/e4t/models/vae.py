@@ -40,7 +40,7 @@ def _norm_act_out(norm, conv, h, engine=False):
     w9 = FN.prepared(conv.weight, "w9_pad64", lambda w: F.pad(w.float(), (0, 0, 0, 0, 0, 0, 0, 64 - co))
                      .permute(2, 3, 0, 1).reshape(9, 64, w.shape[1]).to(torch.bfloat16).contiguous())
     b = FN.prepared(conv.bias, "f32_pad64", lambda t: F.pad(t.float(), (0, 64 - co)).contiguous())
-    y = ops.conv3x3(h, w9, bias=b, out_dtype=torch.float32)                       # (B, H, W, 64) fp32
+    y = FN.conv3x3_any(h, w9, bias=b, out_dtype=torch.float32)                    # (B, H, W, 64) fp32
     return y[..., :co].permute(0, 3, 1, 2).contiguous()
 
 

@@ -161,6 +161,10 @@ class StableDiffusionE4TPipeline:
         domain_embed_scale = self.domain_embed_scale if domain_embed_scale is None else domain_embed_scale
         height = height or self.unet.config.sample_size * self.vae_scale_factor
         width = width or self.unet.config.sample_size * self.vae_scale_factor
+        px = self.unet.latent_multiple * self.vae_scale_factor
+        if height % px or width % px:
+            raise ValueError(f"height and width must be multiples of {px} px (the UNet's down-sampling factor "
+                             f"{self.unet.latent_multiple} times the VAE's {self.vae_scale_factor}); got {height} x {width}")
         assert negative_prompt is None, "negative_prompt is not supported"            # :153
         batch_size = 1 if isinstance(prompt, str) else len(prompt)
         device = self._execution_device

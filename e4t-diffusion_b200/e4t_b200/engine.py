@@ -15,6 +15,7 @@ import torch.nn.functional as F
 
 from . import functional as FN
 from . import ops
+from ._lib import E4TError
 
 PLACEHOLDER_FALLBACK = 49408
 
@@ -253,6 +254,10 @@ class PretrainStep:
             if self.vae is None:
                 raise KeyError("batch has no 'latents' and no VAE is attached to encode 'pixel_values'")
             latents = self.encode_latents(pixel_values, batch.get("vae_noise"))
+        m = self.unet.latent_multiple
+        if latents.shape[-2] % m or latents.shape[-1] % m:
+            raise E4TError(f"latents of {latents.shape[-2]} x {latents.shape[-1]}: the sides must be multiples of the "
+                           f"UNet's down-sampling factor {m}")
         timesteps, input_ids = batch["timesteps"], batch["input_ids"]
         B = latents.shape[0]
         emb = self.text.get_input_embeddings()

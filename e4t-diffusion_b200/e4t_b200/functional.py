@@ -271,6 +271,13 @@ class WOLinearBankFn(torch.autograd.Function):
         return dx, None, None, None
 
 
+def conv3x3_any(x, w9, **kw):
+    """Stride-1 3x3 convolution at any H x W: ops.conv3x3 where its tiled A box covers the size (ops.conv3x3_tiled),
+    ops.conv3x3_im2col elsewhere."""
+    conv = ops.conv3x3 if ops.conv3x3_tiled(x.shape[1], x.shape[2]) else ops.conv3x3_im2col
+    return conv(x, w9, **kw)
+
+
 class Conv3x3Fn(torch.autograd.Function):
     """3x3/s1/p1 convolution on NHWC (+bias +per-image row add (time embedding) +residual).  Backward: dX via the same
     implicit-GEMM kernel with the flipped/transposed taps; pass-through to residual; and, when the fp32 master weight
@@ -280,7 +287,7 @@ class Conv3x3Fn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w9, w9_dgrad, bias, rowgroup, residual, wp=None):
         x = _c(x)
-        y = ops.conv3x3(x, w9, bias=bias, rowgroup=rowgroup, residual=None if residual is None else _c(residual))
+        y = conv3x3_any(x, w9, bias=bias, rowgroup=rowgroup, residual=None if residual is None else _c(residual))
         need_dw = wp is not None and ctx.needs_input_grad[6]
         ctx.save_for_backward(w9_dgrad, x if need_dw else None)
         ctx.has_res = residual is not None
@@ -291,7 +298,7 @@ class Conv3x3Fn(torch.autograd.Function):
         w9_dgrad, x = ctx.saved_tensors
         dy = _c(dy)
         Bn, H, W, Cout = dy.shape
-        dx = ops.conv3x3(dy, w9_dgrad) if ctx.needs_input_grad[0] else None
+        dx = conv3x3_any(dy, w9_dgrad) if ctx.needs_input_grad[0] else None
         db = drow = dw = None
         dy2 = dy.view(-1, Cout)
         if ctx.needs_input_grad[3]:
@@ -324,7 +331,7 @@ class Conv3x3S2Fn(torch.autograd.Function):
         dy = _c(dy)
         Cout = dy.shape[-1]
         up = ops.resample2x(dy, 3)                                              # zero insertion
-        dx = ops.conv3x3(up, w9_dgrad) if ctx.needs_input_grad[0] else None
+        dx = conv3x3_any(up, w9_dgrad) if ctx.needs_input_grad[0] else None
         db = dw = None
         if ctx.needs_input_grad[3]:
             db = ops.colsum_acc(dy.view(-1, Cout), torch.zeros(Cout, device=dy.device, dtype=F32))

@@ -86,6 +86,33 @@ def conv3x3(x, w9, *, bias=None, rowgroup=None, residual=None, out_dtype=BF16, f
     return out
 
 
+def conv3x3_tiled(H, W):
+    """True when conv3x3 (the tiled-box A operand) accepts an H x W output: W divides 128 and the tile's 128 / W rows
+    divide H (or H*W divides 128), or W is a multiple of 128.  Other sizes take conv3x3_im2col; the stride-2
+    convolutions and conv3x3_wgrad choose by the same kind of rule inside the library."""
+    if W > 128:
+        return W % 128 == 0
+    if 128 % W:
+        return False
+    return H % (128 // W) == 0 if H * W >= 128 else 128 % (H * W) == 0
+
+
+def conv3x3_im2col(x, w9, *, bias=None, rowgroup=None, residual=None, out_dtype=BF16, force_bn=0):
+    """conv3x3 with the A operand loaded by TMA in im2col mode (tiles of 128 consecutive pixels across rows and
+    images): any H x W.  Same arguments and result as conv3x3."""
+    assert x.dtype == BF16 and w9.dtype == BF16 and x.is_contiguous() and w9.is_contiguous()
+    Bn, H, W, Cin = x.shape
+    Cout = w9.shape[1]
+    assert w9.shape == (9, Cout, Cin)
+    out = torch.empty((Bn, H, W, Cout), device=x.device, dtype=out_dtype)
+    if residual is not None:
+        assert residual.dtype == BF16 and residual.is_contiguous() and residual.shape == out.shape
+    _lib.call("e4t_conv3x3_im2col_bf16", ptr(x), ptr(w9), ptr(out), c_int(Bn), c_int(H), c_int(W), c_int(Cin),
+              c_int(Cout), c_int(0 if out_dtype == BF16 else 1), ptr(bias), ptr(rowgroup), ptr(residual),
+              c_int(force_bn), stream())
+    return out
+
+
 def conv3x3_s2(x, w9, *, bias=None, force_bn=0, pad_lo=1):
     """3x3 stride-2 convolution on NHWC bf16 (Downsample2D): (B,H,W,Cin) -> (B,H/2,W/2,Cout).
     pad_lo=1: pad 1 on every side; pad_lo=0: one zero row / column on the bottom and right only (diffusers

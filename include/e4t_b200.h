@@ -43,10 +43,15 @@ int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, 
  * bias fp32 [Cout]; rowgroup fp32 [B][Cout] (time-embedding projection added per image); residual bf16 like out. */
 int e4t_conv3x3_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout, int out_mode,
                      const float* bias, const float* rowgroup, const void* residual, int force_bn, void* stream);
+/* e4t_conv3x3_bf16 with the A operand loaded by TMA in im2col mode: a 128-pixel tile is any 128 consecutive output
+ * pixels in NHW order, across row and image boundaries, so any H x W works (Cin % 64 == 0).  Same arguments. */
+int e4t_conv3x3_im2col_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
+                            int out_mode, const float* bias, const float* rowgroup, const void* residual, int force_bn,
+                            void* stream);
 
 /* 3x3 / stride 2 / pad 1 (diffusers Downsample2D.conv, built at e4t/models/unet_2d_blocks.py:801-808): computed at the
  * OUTPUT resolution — the implicit-GEMM A operand is gathered with TMA element strides.  x [B][H][W][Cin] ->
- * out [B][H/2][W/2][Cout]. */
+ * out [B][H/2][W/2][Cout], H and W even.  Output sizes outside e4t_conv3x3_bf16's tiled domain load in im2col mode. */
 int e4t_conv3x3_s2_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                         const float* bias, int force_bn, void* stream);
 /* 3x3 / stride 2 with pad_lo zero rows / columns on the top and left (1 = e4t_conv3x3_s2_bf16; 0 = diffusers
@@ -58,7 +63,8 @@ int e4t_conv3x3_s2p_bf16(const void* x, const void* w, void* out, int B, int H, 
 /* Weight gradient of the 3x3 / stride 1 / pad 1 convolution: dw9[tap][co][ci] += sum dy[b][y][x][co] * x[b][y+ky-1][x+kx-1][ci]
  * (fp32 atomic accumulation; implicit GEMM with 9 taps as the batch dimension, split-K over pixels).  Replaces autograd's
  * conv2d weight gradient when the base UNet is trainable (tuning_e4t.py:139-146; every requires_grad parameter under
- * accelerate's DDP, pretrain_e4t.py:410). */
+ * accelerate's DDP, pretrain_e4t.py:410).  Any H x W: whole-row tiled boxes where W | 64 and H*W % 64 == 0, im2col-mode
+ * loads elsewhere. */
 int e4t_conv3x3_wgrad(const void* x, const void* dy, float* dw9, int B, int H, int W, int Cin, int Cout, void* stream);
 
 /* ---- attention core ------------------------------------------------------------------------------------------ */
