@@ -15,7 +15,8 @@
 // row-group addend, residual) writes each warpgroup's 64 x BN result into its own shared-memory staging buffer, from
 // which TMA stores it (bf16 / fp32) or adds it (fp32 atomic mode) while the warpgroup already runs the next tile's
 // MMAs.  Outputs TMA cannot address (base, row pitch or batch stride not a multiple of 16 bytes) take a register
-// epilogue that stores from the accumulator fragments directly.
+// epilogue that stores from the accumulator fragments directly.  A bf16 output's residual, where TMA can address it,
+// is loaded by TMA into the staging buffer while the tile's MMAs run, so the epilogue adds it from shared memory.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include <stdlib.h>
@@ -113,9 +114,14 @@ __device__ __forceinline__ void gemm_epilogue(const GemmArgs& g, const float* ac
 // Staging layout: sub-tile s holds columns [s * kSubCols, (s + 1) * kSubCols) as 64 rows of 64 bytes; the 16-byte chunk
 // c of row r sits at chunk c ^ ((r >> 1) & 3) (SWIZZLE_64B), so the 8 rows a warp writes per instruction hit 8
 // different bank groups.
-template <int BN, typename OutT>
+// RES_TMA (bf16 output only): the residual tile already sits in the staging buffer, loaded by gemm_residual_load into
+// the bytes each thread's outputs go to; the thread waits on res_bar, adds the bf16 pair it finds there in place of
+// the global read and overwrites it with the output.  The sum and its order are the same, so the output is too.
+template <int BN, typename OutT, bool RES_TMA = false>
 __device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUtensorMap* mapO, const float* acc,
-                                                  uint8_t* stg, int m_t, int n0, int bz, int wg_row, uint32_t bar_id) {
+                                                  uint8_t* stg, int m_t, int n0, int bz, int wg_row, uint32_t bar_id,
+                                                  uint64_t* res_bar = nullptr, uint32_t res_ph = 0) {
+  static_assert(!RES_TMA || sizeof(OutT) == 2, "the TMA-loaded residual fills a bf16 staging buffer");
   constexpr int kEsz = (int)sizeof(OutT);
   constexpr int kSubCols = 64 / kEsz;  // 64-byte sub-tile rows: 32 bf16 or 16 fp32 columns
   constexpr int kSubsPerPass = kStgBytes<BN> / kSubBytes;
@@ -126,15 +132,21 @@ __device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUten
   const int row0 = m_t * kBM + wg_row;
 #pragma unroll
   for (int p = 0; p < kPasses; ++p) {
-    if (tid == 0) tma_store_wait_read<0>();
-    named_bar_sync(bar_id, 128);
+    if constexpr (RES_TMA) {
+      // the load was issued after the previous tile's store had been read out of the buffer
+      if (row0 < g.M) mbar_wait(res_bar, res_ph);
+    } else {
+      if (tid == 0) tma_store_wait_read<0>();
+      named_bar_sync(bar_id, 128);
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = w * 16 + (lane >> 2) + 8 * h;
       const int m = row0 + r;
       if (m >= g.M) continue;
       const float* rg = g.rowgroup ? g.rowgroup + (long long)(m / g.rows_per_group) * g.N : nullptr;
-      const bf16* res = g.residual ? g.residual + (long long)bz * g.res_bstride + (long long)m * g.ldr : nullptr;
+      const bf16* res =
+          !RES_TMA && g.residual ? g.residual + (long long)bz * g.res_bstride + (long long)m * g.ldr : nullptr;
       uint8_t* srow = stg + r * 64;
       const int sw = (r >> 1) & 3;
 #pragma unroll
@@ -143,14 +155,19 @@ __device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUten
         if (sub / kSubsPerPass != p) continue;
         const int n = n0 + 8 * j + 2 * (lane & 3);
         float f0 = acc[4 * j + 2 * h] * g.alpha, f1 = acc[4 * j + 2 * h + 1] * g.alpha;
+        const int byte = (8 * j % kSubCols + 2 * (lane & 3)) * kEsz;
+        uint8_t* dst = srow + (sub % kSubsPerPass) * kSubBytes + ((((byte >> 4) ^ sw)) << 4) + (byte & 15);
         if (n < g.N) {
           const bool two = n + 1 < g.N;
           if (g.bias) { f0 += g.bias[n]; if (two) f1 += g.bias[n + 1]; }
           if (rg) { f0 += rg[n]; if (two) f1 += rg[n + 1]; }
+          if constexpr (RES_TMA) {
+            const float2 rr = unpack_bf16(*reinterpret_cast<const uint32_t*>(dst));
+            f0 += rr.x;
+            if (two) f1 += rr.y;
+          }
           if (res) { f0 += __bfloat162float(res[n]); if (two) f1 += __bfloat162float(res[n + 1]); }
         }
-        const int byte = (8 * j % kSubCols + 2 * (lane & 3)) * kEsz;
-        uint8_t* dst = srow + (sub % kSubsPerPass) * kSubBytes + ((((byte >> 4) ^ sw)) << 4) + (byte & 15);
         if (kEsz == 2) *reinterpret_cast<uint32_t*>(dst) = pack_bf16(f0, f1);
         else *reinterpret_cast<float2*>(dst) = make_float2(f0, f1);
       }
@@ -170,22 +187,38 @@ __device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUten
   }
 }
 
+// The residual tile of one MMA warpgroup's 64 output rows, loaded by TMA (mapR: the residual with mapO's geometry, box
+// and SWIZZLE_64B) into the warpgroup's staging buffer, each element at the byte its output will be written to.  Boxes
+// wholly past N are not issued and not counted; rows past M and columns past N read as zero.
+template <int BN>
+__device__ __forceinline__ void gemm_residual_load(const GemmArgs& g, const CUtensorMap* mapR, uint8_t* stg,
+                                                   uint64_t* bar, int n0, int row0, int bz) {
+  constexpr int kSubCols = 32;
+  const int subs = min(BN / kSubCols, (g.N - n0 + kSubCols - 1) / kSubCols);
+  mbar_expect_tx(bar, (uint32_t)(subs * kSubBytes));
+  for (int s = 0; s < subs; ++s) tma_load_3d(stg + s * kSubBytes, mapR, bar, n0 + s * kSubCols, row0, bz);
+}
+
 // IM2COL: the implicit convolution's pixel operand (conv = 1: A, conv = 2: B) is an im2col-mode tensor map instead
-// of a tiled 4-D box.  A template argument rather than a GemmArgs field, so the kernels every other call runs compile
-// to exactly the code they had without it.
-template <int BN, int AMN, int BMN, bool IM2COL>
+// of a tiled 4-D box.  RES_TMA: the residual of a bf16 staged-epilogue call is TMA-loaded from mapR (host side:
+// out_mode 0, epi_tma, residual addressable by TMA; K-major operands only).  Template arguments rather than GemmArgs
+// fields, so the kernels every other call runs compile to exactly the code they had without them; mapR is the last
+// parameter, so it moves none of the others.
+template <int BN, int AMN, int BMN, bool IM2COL, bool RES_TMA>
 __global__ void __launch_bounds__(kThreads, 1)
 e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                const __grid_constant__ CUtensorMap mapO, const GemmArgs g) {
+                const __grid_constant__ CUtensorMap mapO, const GemmArgs g, const __grid_constant__ CUtensorMap mapR) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // align dynamic smem to 1024 B (SWIZZLE_128B atoms)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   constexpr int kBTileBytes = BN * kBK * 2;
   constexpr int kStageBytes = kATileBytes + kBTileBytes;
   // [stages x {A, B}] [staging of MMA warpgroup 0] [staging of MMA warpgroup 1] [full / empty barriers]
+  // [RES_TMA: residual-loaded barrier of each MMA warpgroup]
   uint8_t* staging = smem + (size_t)g.stages * kStageBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + 2 * kStgBytes<BN>);
   uint64_t* empty_bar = full_bar + g.stages;
+  uint64_t* res_bar = empty_bar + g.stages;
 
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
@@ -195,6 +228,11 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     for (int i = 0; i < g.stages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 256);
+    }
+    if constexpr (RES_TMA) {
+      tma_prefetch_desc(&mapR);
+      mbar_init(&res_bar[0], 1);
+      mbar_init(&res_bar[1], 1);
     }
     fence_mbar_init();
   }
@@ -292,11 +330,13 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     float acc[BN / 2];
     int s = 0;
     uint32_t ph = 0;
+    uint32_t res_ph = 0;
     for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int n_t, m_t, sp, bz;
       gemm_decode(g, t, n_t, m_t, sp, bz);
       const int kc0 = sp * g.kper;
       const int kc1 = min(g.kchunks, kc0 + g.kper);
+      const int row0 = m_t * kBM + wg_row;
       int prev = -1;
       for (int kc = kc0; kc < kc1; ++kc) {
         mbar_wait(&full_bar[s], ph);
@@ -310,6 +350,15 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                                    (kc > kc0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         reg_fence<BN / 2>(acc);
+        if constexpr (RES_TMA) {
+          // with the tile's first MMAs under way, the thread that committed the previous tile's store waits until
+          // TMA has read the staging buffer out, then has TMA fill it with this tile's residual
+          if (kc == kc0 && (threadIdx.x & 127) == 0 && row0 < g.M) {
+            tma_store_wait_read<0>();
+            gemm_residual_load<BN>(g, &mapR, staging + (wg - 1) * kStgBytes<BN>, &res_bar[wg - 1], n_t * BN, row0, bz);
+          }
+          __syncwarp();
+        }
         // the MMAs of the previous k-chunk have retired: its stage can be refilled
         wgmma_wait<1>();
         reg_fence<BN / 2>(acc);
@@ -323,7 +372,11 @@ e4t_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
       wgmma_wait<0>();
       reg_fence<BN / 2>(acc);
       if (prev >= 0) mbar_arrive(&empty_bar[prev]);
-      if (!g.epi_tma) {
+      if constexpr (RES_TMA) {
+        gemm_epilogue_tma<BN, bf16, true>(g, &mapO, acc, staging + (wg - 1) * kStgBytes<BN>, m_t, n_t * BN, bz, wg_row,
+                                          wg, &res_bar[wg - 1], res_ph);
+        if (row0 < g.M) res_ph ^= 1u;
+      } else if (!g.epi_tma) {
         gemm_epilogue<BN, AMN, BMN>(g, acc, m_t, n_t * BN, bz, wg_row);
       } else {
         uint8_t* stg = staging + (wg - 1) * kStgBytes<BN>;
@@ -403,42 +456,44 @@ static int auto_splits(int N, long m_tiles_x_batch, bool b_mn, int kchunks) {
   return best;
 }
 
-template <int BN, int AMN, int BMN, bool IM2COL>
-static int launch_gemm_t(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, GemmArgs& g, int grid,
-                         cudaStream_t stream) {
+template <int BN, int AMN, int BMN, bool IM2COL, bool RES_TMA>
+static int launch_gemm_t(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, const CUtensorMap& mR,
+                         GemmArgs& g, int grid, cudaStream_t stream) {
   constexpr int stage_bytes = kATileBytes + BN * kBK * 2;
+  constexpr int res_bars = RES_TMA ? 2 : 0;
   // the ring gets what the two staging buffers, the barriers and the 1 KiB alignment slack leave of 227 KiB
-  int stages = (227 * 1024 - 1024 - 2 * kStgBytes<BN> - 16 * (int)sizeof(uint64_t)) / stage_bytes;
+  int stages = (227 * 1024 - 1024 - 2 * kStgBytes<BN> - (16 + res_bars) * (int)sizeof(uint64_t)) / stage_bytes;
   if (stages > 8) stages = 8;
   if (stages > g.kper) stages = g.kper < 2 ? 2 : g.kper;
   g.stages = stages;
-  const size_t smem = (size_t)stages * stage_bytes + 2 * kStgBytes<BN> + 2 * stages * sizeof(uint64_t) + 1024;
+  const size_t smem =
+      (size_t)stages * stage_bytes + 2 * kStgBytes<BN> + (2 * stages + res_bars) * sizeof(uint64_t) + 1024;
   static bool attr_set = false;
   if (!attr_set) {
-    E4T_CUDA(cudaFuncSetAttribute(e4t_gemm_kernel<BN, AMN, BMN, IM2COL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  227 * 1024));
+    E4T_CUDA(cudaFuncSetAttribute(e4t_gemm_kernel<BN, AMN, BMN, IM2COL, RES_TMA>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  e4t_gemm_kernel<BN, AMN, BMN, IM2COL><<<grid, kThreads, smem, stream>>>(mA, mB, mO, g);
+  e4t_gemm_kernel<BN, AMN, BMN, IM2COL, RES_TMA><<<grid, kThreads, smem, stream>>>(mA, mB, mO, g, mR);
   E4T_COUNT_LAUNCH();
   E4T_LAUNCH_CHECK();
   return 0;
 }
 
-template <int AMN, int BMN, bool IM2COL>
-static int launch_gemm_bn(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, GemmArgs& g, int grid,
-                          cudaStream_t stream) {
+template <int AMN, int BMN, bool IM2COL, bool RES_TMA = false>
+static int launch_gemm_bn(const CUtensorMap& mA, const CUtensorMap& mB, const CUtensorMap& mO, const CUtensorMap& mR,
+                          GemmArgs& g, int grid, cudaStream_t stream) {
   switch (g.BN) {
-    case 64: return launch_gemm_t<64, AMN, BMN, IM2COL>(mA, mB, mO, g, grid, stream);
-    case 128: return launch_gemm_t<128, AMN, BMN, IM2COL>(mA, mB, mO, g, grid, stream);
-    case 192: return launch_gemm_t<192, AMN, BMN, IM2COL>(mA, mB, mO, g, grid, stream);
-    case 256: return launch_gemm_t<256, AMN, BMN, IM2COL>(mA, mB, mO, g, grid, stream);
+    case 64: return launch_gemm_t<64, AMN, BMN, IM2COL, RES_TMA>(mA, mB, mO, mR, g, grid, stream);
+    case 128: return launch_gemm_t<128, AMN, BMN, IM2COL, RES_TMA>(mA, mB, mO, mR, g, grid, stream);
+    case 192: return launch_gemm_t<192, AMN, BMN, IM2COL, RES_TMA>(mA, mB, mO, mR, g, grid, stream);
+    case 256: return launch_gemm_t<256, AMN, BMN, IM2COL, RES_TMA>(mA, mB, mO, mR, g, grid, stream);
   }
   if constexpr (!BMN) {
     switch (g.BN) {
-      case 96: return launch_gemm_t<96, AMN, 0, IM2COL>(mA, mB, mO, g, grid, stream);
-      case 160: return launch_gemm_t<160, AMN, 0, IM2COL>(mA, mB, mO, g, grid, stream);
-      case 224: return launch_gemm_t<224, AMN, 0, IM2COL>(mA, mB, mO, g, grid, stream);
+      case 96: return launch_gemm_t<96, AMN, 0, IM2COL, RES_TMA>(mA, mB, mO, mR, g, grid, stream);
+      case 160: return launch_gemm_t<160, AMN, 0, IM2COL, RES_TMA>(mA, mB, mO, mR, g, grid, stream);
+      case 224: return launch_gemm_t<224, AMN, 0, IM2COL, RES_TMA>(mA, mB, mO, mR, g, grid, stream);
     }
   }
   return e4t_set_error("e4t_gemm_bf16: unsupported tile width BN=%d (b_mn=%d)", g.BN, BMN);
@@ -464,18 +519,36 @@ static int launch_gemm(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs& g
     uint32_t box[3] = {(uint32_t)(64 / esz), 64, 1};
     if (int e = e4t_tmap_encode(&mO, g.out, 3, dims, str, box, esz, 64)) return e;
   }
+  // A bf16 staged epilogue's residual is TMA-loaded into the staging buffer under the MMAs when TMA can address it as
+  // it addresses the output (the same conditions on base, row pitch and batch stride); fp32 outputs, the register
+  // epilogue and other residuals read it from global memory in the epilogue.  Residual calls all have K-major
+  // operands, so only those kernels are built with the load.
+  const bool res_tma = g.epi_tma && g.out_mode == 0 && g.residual && !g.a_mn && !g.b_mn &&
+                       ((uintptr_t)g.residual % 16) == 0 && (g.ldr * 2) % 16 == 0 && g.ldr >= g.N &&
+                       (g.batch == 1 || (g.res_bstride > 0 && (g.res_bstride * 2) % 16 == 0));
+  CUtensorMap mR;
+  memset(&mR, 0, sizeof(mR));
+  if (res_tma) {
+    const uint64_t bs = g.batch == 1 ? (uint64_t)g.ldr * g.M : (uint64_t)g.res_bstride;
+    uint64_t dims[3] = {(uint64_t)g.N, (uint64_t)g.M, (uint64_t)g.batch};
+    uint64_t str[2] = {(uint64_t)g.ldr * 2, bs * 2};
+    uint32_t box[3] = {32, 64, 1};
+    if (int e = e4t_tmap_encode(&mR, g.residual, 3, dims, str, box, 2, 64)) return e;
+  }
   const long total = (long)g.batch * g.splits * g.m_tiles * g.n_tiles;
   int grid = (int)(total < num_sms() ? total : num_sms());
   if (grid < 1) return 0;
   // the implicit convolutions load A K-major (wgrad: both operands MN-major, set in a_mn / b_mn)
   if (im2col)
-    return g.a_mn ? launch_gemm_bn<1, 1, true>(mA, mB, mO, g, grid, stream)
-                  : launch_gemm_bn<0, 0, true>(mA, mB, mO, g, grid, stream);
+    return g.a_mn ? launch_gemm_bn<1, 1, true>(mA, mB, mO, mR, g, grid, stream)
+           : res_tma ? launch_gemm_bn<0, 0, true, true>(mA, mB, mO, mR, g, grid, stream)
+                     : launch_gemm_bn<0, 0, true>(mA, mB, mO, mR, g, grid, stream);
   if (g.a_mn)
-    return g.b_mn ? launch_gemm_bn<1, 1, false>(mA, mB, mO, g, grid, stream)
-                  : launch_gemm_bn<1, 0, false>(mA, mB, mO, g, grid, stream);
-  return g.b_mn ? launch_gemm_bn<0, 1, false>(mA, mB, mO, g, grid, stream)
-                : launch_gemm_bn<0, 0, false>(mA, mB, mO, g, grid, stream);
+    return g.b_mn ? launch_gemm_bn<1, 1, false>(mA, mB, mO, mR, g, grid, stream)
+                  : launch_gemm_bn<1, 0, false>(mA, mB, mO, mR, g, grid, stream);
+  return g.b_mn  ? launch_gemm_bn<0, 1, false>(mA, mB, mO, mR, g, grid, stream)
+         : res_tma ? launch_gemm_bn<0, 0, false, true>(mA, mB, mO, mR, g, grid, stream)
+                   : launch_gemm_bn<0, 0, false>(mA, mB, mO, mR, g, grid, stream);
 }
 
 extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K, int batch, int a_mn,

@@ -1,6 +1,6 @@
 """Per-call inventory and A/B timing of the GEMM / implicit-convolution engine over one pre-training step.
 
-    python tools/gemm_ab.py [--lib PATH ...] [--batch 16] [--iters 15] [--out FILE]
+    python tools/gemm_ab.py [--lib PATH ...] [--batch 16] [--iters 15] [--without-residual] [--out FILE]
 
 Runs one eager pre-training step (bench.py's models and inputs, after one warm-up step) with ops.gemm, ops.conv3x3,
 ops.conv3x3_s2 and ops.conv3x3_wgrad wrapped, and records every call: shapes, operand majors, output dtype and mode,
@@ -11,6 +11,9 @@ over --iters launches) and weighted by its call count.
 Every --lib names a libe4t_b200.so; the first one runs the step.  With several, the libraries are loaded side by side
 and timed alternately, launch by launch, and their outputs are compared on the same inputs.  Card name, power limit and
 SM clock are read in the same run.  Needs a GPU; fails without one.
+
+--without-residual replays every call that adds a residual a second time with residual=None, alternating with the
+original call on the same inputs, and reports per call and call-weighted per step what adding the residual costs.
 """
 import argparse
 import ctypes
@@ -142,7 +145,16 @@ def describe(key):
     return d
 
 
+def out_elems(row):
+    """Elements of the call's output (and of its residual)."""
+    if row["op"] == "gemm":
+        return row["M"] * row["N"] * row["batch"]
+    s = 2 if row["op"] == "conv3x3_s2" else 1
+    return row["B"] * (row["H"] // s) * (row["W"] // s) * row["Cout"]
+
+
 def replay_fn(key, g):
+    """run(drop=()) replays the call on fresh seeded inputs, leaving out the keyword arguments named in drop."""
     from e4t_b200 import ops
     name, args, kw = key
     a = [make(s, g) if s[0] == "T" else s[1] for s in args]
@@ -150,10 +162,10 @@ def replay_fn(key, g):
     out = k.get("out")
     fn = getattr(ops, name)
 
-    def run():
+    def run(drop=()):
         if out is not None and k.get("accumulate"):
             out.zero_()
-        r = fn(*a, **k)
+        r = fn(*a, **{n: v for n, v in k.items() if n not in drop})
         return out if r is None else r
     return run
 
@@ -168,6 +180,8 @@ def main():
     ap.add_argument("--lib", action="append", default=[], help="libe4t_b200.so to time (repeat to A/B; first runs the step)")
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--iters", type=int, default=15)
+    ap.add_argument("--without-residual", action="store_true",
+                    help="also time every residual call with residual=None and report what the residual costs")
     ap.add_argument("--out", default=None, help="also write the JSON report here")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -197,7 +211,10 @@ def main():
     for i, (key, count) in enumerate(calls.items()):
         g = torch.Generator(device="cuda").manual_seed(1000 + i)
         run = replay_fn(key, g)
-        outs, times = [], [[] for _ in handles]
+        row = describe(key)
+        row["count"] = count
+        nores = args.without_residual and row.get("residual", False)
+        outs, times, times_nores = [], [[] for _ in handles], [[] for _ in handles]
         for h in handles:
             _lib._lib = h
             outs.append(run().clone())
@@ -207,10 +224,16 @@ def main():
                 t = timed(run)
                 if it:
                     times[li].append(t)
-        row = describe(key)
-        row["count"] = count
+                if nores:
+                    t = timed(lambda: run(drop=("residual",)))
+                    if it:
+                        times_nores[li].append(t)
         for li in range(len(handles)):
             row[f"lib{li}"] = stats(times[li])
+            if nores:
+                row[f"lib{li}_without_residual"] = stats(times_nores[li])
+                row[f"lib{li}_residual_cost_ms"] = round(row[f"lib{li}"]["median_ms"]
+                                                         - row[f"lib{li}_without_residual"]["median_ms"], 4)
         if len(handles) > 1:
             a, b = outs[0].float(), outs[1].float()
             row["max_abs_diff_vs_lib0"] = (a - b).abs().max().item()
@@ -227,6 +250,16 @@ def main():
         tot[f"lib{li}_ms_per_step"] = round(sum(r["count"] * r[f"lib{li}"]["median_ms"] for r in rows), 3)
         k640 = [r for r in rows if r["op"] == "gemm" and r["K"] <= 640]
         tot[f"lib{li}_gemm_K_le_640_ms_per_step"] = round(sum(r["count"] * r[f"lib{li}"]["median_ms"] for r in k640), 3)
+        if args.without_residual:
+            res = [r for r in rows if r.get("residual")]
+            tot[f"lib{li}_residual_calls_ms_per_step"] = round(
+                sum(r["count"] * r[f"lib{li}"]["median_ms"] for r in res), 3)
+            tot[f"lib{li}_residual_cost_ms_per_step"] = round(
+                sum(r["count"] * r[f"lib{li}_residual_cost_ms"] for r in res), 3)
+    if args.without_residual:
+        res = [r for r in rows if r.get("residual")]
+        tot["residual_calls_per_step"] = sum(r["count"] for r in res)
+        tot["residual_elements_per_step"] = sum(r["count"] * out_elems(r) for r in res)
     tot["flops_per_step"] = sum(r["count"] * r["flops"] for r in rows)
     report["totals"] = tot
     report["card_after"] = card()
@@ -236,7 +269,8 @@ def main():
         with open(args.out, "w") as f:
             f.write(txt)
     # table: one line per distinct call, heaviest first
-    print(f"{'op':14s} {'shape':44s} {'epi':22s} {'n':>3s} " + " ".join(f"{'lib%d ms' % i:>9s}" for i in range(len(handles))))
+    print(f"{'op':14s} {'shape':44s} {'epi':22s} {'n':>3s} " + " ".join(f"{'lib%d ms' % i:>9s}" for i in range(len(handles)))
+          + ("".join(f" {'lib%d res' % i:>9s}" for i in range(len(handles))) if args.without_residual else ""))
     for r in sorted(rows, key=lambda r: -r["count"] * r["lib0"]["median_ms"]):
         shp = (f"{r['M']}x{r['N']}x{r['K']} b{r['batch']} {'T' if r['a_mn'] else 'N'}{'T' if r['b_mn'] else 'N'}"
                if r["op"] == "gemm" else f"{r['B']}x{r['H']}x{r['W']} {r['Cin']}->{r['Cout']}")
