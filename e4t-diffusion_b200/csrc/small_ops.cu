@@ -24,6 +24,9 @@ __device__ __forceinline__ float act_df(float x, int mode) {
     return cdf + x * 0.3989422804014327f * __expf(-0.5f * x * x);
   }
   if (mode == 1) {
+    // beyond |x| = 1e30 the sigmoid is exactly 0 or 1 in fp32; the clamp keeps 1.702x finite, so the product below is
+    // 0 * finite instead of 0 * inf = NaN for |x| > 2e38
+    x = fminf(fmaxf(x, -1e30f), 1e30f);
     const float s = 1.f / (1.f + __expf(-1.702f * x));
     return s * (1.f + 1.702f * x * (1.f - s));
   }

@@ -80,7 +80,8 @@ class BasicTransformerBlock(nn.Module):
 
 
 # the fp32 score matrix of one image is N² · 4 bytes (64 MiB at a 64 x 64 latent); images are processed in chunks
-# whose scores stay under this bound
+# whose scores stay under this bound, and never fewer than one image per chunk: above 128 x 128 latent tokens one image
+# is already over it (1.2 GB of scores + 0.6 GB of bf16 probabilities at 1088 x 1024 px, 2.4 + 1.2 GB at 1024 x 1536)
 ATTN_SCORE_BYTES = 1 << 30
 
 

@@ -839,3 +839,123 @@ def test_replay_every_recorded_call(inventory, op):
     print(f"[replay {op}] {len(keys)} signatures; worst global error {worst_g:.2f}x its bound, worst block "
           f"{worst_b:.2f}x the global bound ({time.time() - t0:.0f} s)")
     assert not failures, "\n".join(failures)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the attention and softmax signatures again, at peaked scores
+# ---------------------------------------------------------------------------------------------------------------------
+PEAKED_OPS = ("attn_fwd", "attn_bwd", "attn_small_fwd", "attn_small_bwd", "softmax_rows")
+
+
+def _refill_peaked(c, g):
+    """q / k of an attention call (or the fp32 scores of a softmax_rows call) refilled by the peaked-score generator of
+    test_attention_numerics_gpu.py, the sink keys' V rows zeroed; returns a line with the Δ / σ reached."""
+    import test_attention_numerics_gpu as AN
+    if c.name == "softmax_rows":
+        # the rows spread over 9 generator slots: every (Δ, σ) pair of the generator's cycles
+        x = c["x"]
+        n = x.shape[-1]
+        x2 = x.view(-1, n) if x.dim() > 2 else x
+        rows, slots, dh = x2.shape[0], 9, 64
+        per = -(-rows // slots)
+        q, k, peaked, sinks = AN.peaked_qk(slots, per, n, 1, dh, dh ** -0.5, g)
+        q, k = q.to(torch.bfloat16), k.to(torch.bfloat16)
+        x2.copy_(((q.double() @ k.double().transpose(1, 2)) * dh ** -0.5).reshape(-1, n)[:rows])
+        dmin, sig = AN.achieved(q, k, 1, dh ** -0.5, peaked, sinks)
+        return f"Δ ≥ {dmin:.1f} nats, flat-row σ {sig[0]:.2f} to {sig[1]:.2f}"
+    q, k, v, heads = c["q"], c["k"], c["v"], c["heads"]
+    B, N, C = q.shape
+    M = k.shape[1]
+    dh = C // heads
+    scale = _attn_scale(c, C, heads)
+    qg, kg, peaked, sinks = AN.peaked_qk(B, N, M, heads, dh, scale, g)
+    q.copy_(qg)
+    k.copy_(kg)
+    for i, j in enumerate(sinks):
+        b, h = divmod(i, heads)
+        v[b, j, h * dh:(h + 1) * dh] = 0
+    dmin, sig = AN.achieved(q, k, heads, scale, peaked, sinks, bool(c.kw.get("causal", False)))
+    return f"Δ ≥ {dmin:.1f} nats, flat-row σ {sig[0]:.2f} to {sig[1]:.2f}"
+
+
+def _peaked_attention(c, sig, failures):
+    """Runs one attention call against test_attention_numerics_gpu.reference: O elementwise and the LSE per row to
+    their derived bounds (forward), the per-row gradient bound (backward), plus the replay's tensor and block bounds."""
+    import test_attention_numerics_gpu as AN
+    q, k, v, heads = c["q"], c["k"], c["v"], c["heads"]
+    B, N, C = q.shape
+    dh = C // heads
+    scale = _attn_scale(c, C, heads)
+    causal = bool(c.kw.get("causal", False))
+    bwd = c.name in ("attn_bwd", "attn_small_bwd")
+    refs, (o_bound, lse_bound), noise = AN.reference(q, k, v, c["do"] if bwd else None, heads, scale, causal)
+    checks, rows = [], []
+    if bwd:
+        c["o"].copy_(refs[0])
+        c["lse"].copy_(refs[1])
+        for n in ("dq", "dk", "dv"):
+            c.nan_(n)
+        got = c.run()
+        for n, t, r in zip(("dq", "dk", "dv"), got, refs[2:]):
+            checks.append(Check(n, t, r, 1e-2, block=(64, dh), unit="(image * tokens / 64 + token block, head)"))
+            rw, nrows, at = AN.row_error(t, r, heads, noise[n], 1e-2)
+            rows.append((n, rw / 1e-2, f"{n}: worst row {rw / 1e-2:.2f}x over the {nrows} of {t.numel() // dh} rows "
+                                       f"above their noise (at {at})"))
+            if rw > LOCAL * 1e-2:
+                failures.append(f"{sig}: {n} row (token, head) {at} error {rw:.2e} (bound {LOCAL * 1e-2:.1e})")
+    else:
+        o, lse = c.run()
+        checks.append(Check("o", o, refs[0], 6e-3, block=(64, dh), unit="(image * N / 64 + query block, head)"))
+        for n, t, r, bnd in (("o elementwise", o, refs[0], o_bound), ("lse per row", lse, refs[1], lse_bound)):
+            w, _ = AN.elementwise(t, r, bnd)
+            rows.append((n, w, f"{n}: worst {w:.2f}x its derived bound"))
+            if w > 1:
+                failures.append(f"{sig}: {n} {w:.2f}x its derived bound")
+    return checks, rows
+
+
+def test_replay_attention_peaked(inventory):
+    """Every recorded attention and softmax_rows signature with q / k (or the scores) from the peaked-score generator:
+    sinks Δ = 8 / 24 / 48 nats above the row, other logits spread by σ = 1 / 3 / 6 nats, half the query rows flat, the
+    sinks' V rows zero.  The replay's bounds, plus O elementwise and the LSE per row to derived bounds, and each query
+    row of dQ and key row of dK / dV within 4x the bound of its own fp64 RMS where its derived noise allows
+    (test_attention_numerics_gpu.py)."""
+    keys = [k for k in inventory if k[0] in PEAKED_OPS]
+    assert {k[0] for k in keys} >= {"attn_fwd", "attn_bwd", "attn_small_fwd", "softmax_rows"}
+    failures, worst = [], {}
+    for i, key in enumerate(keys):
+        g = torch.Generator(device="cuda").manual_seed(5000 + i)
+        c = Call(key, g)
+        reached = _refill_peaked(c, g)
+        sig = describe(key)
+        if key[0] == "softmax_rows":        # (its handler would redraw the scores)
+            if c["out"] is not None:
+                c.nan_("out")
+            checks, rows = [Check("out", c.run(), torch.softmax(_d(c["x"]), -1), 4e-3)], []
+        else:
+            checks, rows = _peaked_attention(c, sig, failures)
+        bad = c.guards_intact()
+        if bad:
+            failures.append(f"{sig}: wrote outside the logical extent of {bad}")
+        line = [reached]
+        for chk in checks:
+            finite, glob, wb, where = evaluate(chk)
+            w = worst.setdefault((key[0], chk.label), [0.0, 0.0])
+            w[0], w[1] = max(w[0], glob / chk.bound), max(w[1], wb / chk.bound)
+            line.append(f"{chk.label}: global {glob / chk.bound:.2f}x, block {wb / chk.bound:.2f}x")
+            if not finite:
+                failures.append(f"{sig}: {chk.label} has non-finite elements")
+            elif glob > chk.bound or wb > LOCAL * chk.bound:
+                failures.append(f"{sig}: {chk.label} error {glob:.2e} (bound {chk.bound:.1e}); worst {chk.unit} "
+                                f"at {where}: {wb:.2e} (bound {LOCAL * chk.bound:.1e})")
+        for n, r, text in rows:
+            w = worst.setdefault((key[0], n), [0.0, 0.0])
+            w[1] = max(w[1], r)
+            line.append(text)
+        print(f"[peaked {sig}] " + "; ".join(line))
+        del c
+        _free()
+    for (op, label), (gw, bw) in sorted(worst.items()):
+        print(f"[peaked replay {op} {label}] worst " + (f"global {gw:.2f}x, block / row / element {bw:.2f}x" if gw
+                                                        else f"{bw:.2f}x") + " the bound")
+    assert not failures, "\n".join(failures)
