@@ -17,9 +17,10 @@
 // same kernel stages dSᵀ in shared memory and reduces dQ += dS·K into an fp32 buffer with atomics.  The two-kernel form
 // computes dQ in a kernel of its own (CTA = 64 queries, loop over key blocks).
 //
-// Which shapes run here: everything except the non-causal forward and single-pass backward with dh = 40 and N, M
-// multiples of 128 and >= 512 (the 4096-token self-attention), which the entry points below hand to the warpgroup
-// kernels of attention_wgmma.cu unless a switch (see "Runtime switches") keeps them here.
+// Which shapes run here: everything except the non-causal forward and single-pass backward with dh = 40 or 80 and N, M
+// multiples of 128 and >= 512 (the 4096-token level-0 and 1024-token level-1 self-attention; for dh = 80 only grids of
+// at least half as many 128-query CTAs as SMs), which the entry points below hand to the warpgroup kernels of
+// attention_wgmma.cu unless a switch (see "Runtime switches") keeps them here.
 #include "attention.cuh"
 #include <math.h>
 #include <stdlib.h>
@@ -631,8 +632,8 @@ static int env_int(const char* name, int dflt) {
   return (e && *e) ? atoi(e) : dflt;
 }
 
-static bool attn_use_wgmma(int N, int M, int dh) {
-  if (!attn_wgmma_shape_ok(N, M, dh) || !env_int("E4T_ATTN_WGMMA", 1)) return false;
+static bool attn_use_wgmma(int B, int H, int N, int M, int dh) {
+  if (!attn_wgmma_shape_ok(B, H, N, M, dh) || !env_int("E4T_ATTN_WGMMA", 1)) return false;
   for (const char* v : {"E4T_ATTN_FWD2", "E4T_ATTN_FWD_PT", "E4T_ATTN_CG", "E4T_ATTN_BWD_FUSED", "E4T_ATTN_BWD_BQ",
                         "E4T_ATTN_BWD_STAGES"})
     if (getenv(v)) return false;
@@ -686,7 +687,7 @@ extern "C" int e4t_attn_fwd(const void* Q, const void* K, const void* V, void* O
   if (int e = attn_common_checks(dh, ldq, ldk, ldv)) return e;
   AttnArgs a = attn_args(Q, K, V, B, H, N, M, dh, ldq, q_bs, ldk, k_bs, ldv, v_bs, scale);
   a.O = (bf16*)O; a.ldo = ldo; a.o_bs = o_bs; a.LSE = LSE;
-  if (attn_use_wgmma(N, M, dh)) return attn_wgmma_fwd(a, st);
+  if (attn_use_wgmma(B, H, N, M, dh)) return attn_wgmma_fwd(a, st);
   a.stages = 2;
   int warps = 4, cap = 0;
   if (const char* e = getenv("E4T_ATTN_FWD2")) {
@@ -751,7 +752,7 @@ static int attn_bwd_impl(const void* Q, const void* K, const void* V, const void
   const dim3 gkv(cdiv(M, kBlk), H, B), gq(cdiv(N, kBlk), H, B);
   const int dp = attn_dp(dh);
   int r = -1;
-  const bool wg = fused && !causal && attn_use_wgmma(N, M, dh);
+  const bool wg = fused && !causal && attn_use_wgmma(B, H, N, M, dh);
   if (wg) r = attn_wgmma_bwd(a, st);
 #define E4T_BWD_KV(D, BQ, S)                                                                                     \
   {                                                                                                              \

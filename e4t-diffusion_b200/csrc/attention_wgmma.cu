@@ -1,11 +1,17 @@
-// e4t — warpgroup-level attention for the long non-causal self-attention of the SD-v1.4 UNet (N = M = 4096, 8 heads of
-// 40): wgmma.mma_async from SWIZZLE_128B shared-memory tiles that TMA fills, fp32 accumulators in registers.
-// Same function, arguments and outputs as the mma.sync kernels of attention.cu, which keep every other shape.
+// e4t — warpgroup-level attention for the long non-causal self-attention of the SD-v1.4 UNet: level 0 (N = M = 4096,
+// 8 heads of 40) and level 1 (N = M = 1024, 8 heads of 80).  wgmma.mma_async from SWIZZLE_128B shared-memory tiles
+// that TMA fills, fp32 accumulators in registers.  Same function, arguments and outputs as the mma.sync kernels of
+// attention.cu, which keep every other shape.
 //
-// Loading: a head slice is dh = 40 bf16 (80 B) wide inside a token row.  Q/K/V/dO are described to TMA as the 4-D
-// tensor (dh, H, tokens, B) with a box of 64 x 1 x rows x 1: columns >= dh are out of bounds and arrive as zeros, so a
-// tile is rows x 128 B, swizzled, with no neighbouring head in the padding.  Products over the head dim take
-// ceil(dh / 16) k-steps; products whose N is the head dim use an instruction of exactly N = dh.
+// Which shapes run here (attn_wgmma_shape_ok): dh = 40 or 80, N and M multiples of 128 and >= 512; for dh = 80 also a
+// grid of (N / 128) x H x B CTAs of at least half the device's SM count.
+//
+// Loading: a head slice is dh bf16 wide inside a token row.  Q/K/V/dO are described to TMA as the 4-D tensor
+// (dh, H, tokens, B) with a box of 64 x 1 x rows x 1, loaded once per 64-column panel (x = 0, and x = 64 for dh = 80):
+// columns >= dh are out of bounds and arrive as zeros, so a panel is rows x 128 B, swizzled, with no neighbouring head
+// in the padding.  A tile is its panels one after the other.  Products over the head dim take ceil(dh / 16) k-steps,
+// the fifth one (dh = 80) reading the second panel; products whose N is the head dim use an instruction of exactly
+// N = dh, which reads an MN-major operand's second panel at the descriptor's leading byte offset.
 //
 // Forward, CTA = (128 queries, head, batch), 384 threads: warpgroup 0 is the producer (one thread issues TMA into a
 // ring of K/V blocks of 128 keys), warpgroups 1 and 2 own 64 query rows each.  S = Q·Kᵀ from shared memory, online
@@ -24,13 +30,52 @@
 
 static constexpr int kWgThreads = 384;
 static constexpr int kFwdStages = 3;     // K/V ring of the forward
-static constexpr int kBwdStages = 3;     // Q/dO ring of the backward
-static constexpr int kTile128 = 128 * 128;   // bytes of a 128-row tile
-static constexpr int kTile64 = 64 * 128;     // bytes of a 64-row tile
+static constexpr int kTile128 = 128 * 128;   // bytes of a 128-row panel
+static constexpr int kTile64 = 64 * 128;     // bytes of a 64-row panel
+static constexpr size_t kMaxSmem = 227 * 1024;
+
+// k-step k (16 columns of the head dim) of a K-major tile whose 64-column panels are `panel` bytes apart, in
+// descriptor units
+__device__ __forceinline__ constexpr uint64_t kstep(int k, uint32_t panel) {
+  return (uint64_t)((k / 4) * (panel >> 4) + 2 * (k % 4));
+}
 
 __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
   return p + ((1024u - (smem_u32(p) & 1023u)) & 1023u);
 }
+
+// Shared-memory layouts, used by the kernels and by the host for the launch size
+template <int DH>
+struct FwdSmem {
+  static constexpr int P = (DH + 63) / 64;                 // 64-column panels of a tile
+  static constexpr uint32_t kTile = P * kTile128;          // Q, K or V: 128 rows
+  static constexpr uint32_t kStage = 2 * kTile;            // K, V
+  static constexpr uint32_t kOffBar = kTile + kFwdStages * kStage;
+  static constexpr size_t bytes = 1024 + kOffBar + 8 * (1 + 2 * kFwdStages);
+  // leading byte offset of the MN-major V: the stride between its panels (a single panel leaves it unread)
+  static constexpr uint32_t kLboV = P > 1 ? kTile128 : kTile64;
+  static_assert(bytes <= kMaxSmem, "forward shared memory");
+};
+
+template <int DH>
+struct BwdSmem {
+  static constexpr int P = (DH + 63) / 64, BQ = 64;
+  static constexpr int kStages = P > 1 ? 2 : 3;             // Q/dO ring; a third two-panel stage does not fit
+  static constexpr uint32_t kKV = P * kTile128;            // K or V: 128 rows
+  static constexpr uint32_t kQ = P * kTile64;              // Q or dO: 64 rows
+  static constexpr uint32_t kStage = 2 * kQ;               // Q, dO
+  static constexpr uint32_t kOffQ = 2 * kKV;               // after K, V
+  static constexpr uint32_t kOffdS = kOffQ + kStages * kStage;   // [2][128 keys][64 queries] bf16
+  static constexpr uint32_t kOffdQ = kOffdS + 2 * kTile128;      // [2][64 queries][DH] fp32
+  static constexpr uint32_t kdQBytes = BQ * DH * 4;
+  static constexpr uint32_t kOffL = kOffdQ + 2 * kdQBytes;       // [stages][64] LSE, [stages][64] D
+  static constexpr uint32_t kOffBar = kOffL + kStages * 2 * BQ * 4;
+  static constexpr size_t bytes = 1024 + kOffBar + 8 * (1 + 2 * kStages + 4);
+  // leading byte offset of the MN-major K in dQ = dS·K (a single panel leaves it unread)
+  static constexpr uint32_t kLboK = P > 1 ? kTile128 : kTile64;
+  static_assert(kOffdQ % 128 == 0 && kdQBytes % 128 == 0 && kOffL % 16 == 0 && kOffBar % 8 == 0, "smem layout");
+  static_assert(bytes <= kMaxSmem, "backward shared memory");
+};
 
 // =============================================================================================
 // Forward
@@ -72,11 +117,12 @@ template <int DH>
 __global__ void __launch_bounds__(kWgThreads, 1)
 attn_wgmma_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                       const __grid_constant__ CUtensorMap mapV, const AttnArgs a) {
+  using L = FwdSmem<DH>;
   constexpr int KS = (DH + 15) / 16, NO = DH;
-  constexpr uint32_t kStage = 2 * kTile128;
+  constexpr uint32_t kStage = L::kStage;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = align1024(smem_raw);   // [Q 128 x 128 B][stages x (K, V)]
-  uint64_t* q_bar = reinterpret_cast<uint64_t*>(smem + kTile128 + kFwdStages * kStage);
+  uint8_t* smem = align1024(smem_raw);   // [Q][stages x (K, V)], each P panels of 128 x 128 B
+  uint64_t* q_bar = reinterpret_cast<uint64_t*>(smem + L::kOffBar);
   uint64_t* full_bar = q_bar + 1;
   uint64_t* empty_bar = full_bar + kFwdStages;
   const int wg = threadIdx.x >> 7;
@@ -98,16 +144,20 @@ attn_wgmma_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
   if (wg == 0) {
     setmaxnreg_dec<24>();
     if (threadIdx.x != 0) return;
-    mbar_expect_tx(q_bar, kTile128);
-    tma_load_4d(smem, &mapQ, q_bar, 0, h, q0, b);
+    mbar_expect_tx(q_bar, L::kTile);
+#pragma unroll
+    for (int pn = 0; pn < L::P; ++pn) tma_load_4d(smem + pn * kTile128, &mapQ, q_bar, 64 * pn, h, q0, b);
     int s = 0;
     uint32_t ph = 0;
     for (int j = 0; j < nblk; ++j) {
       mbar_wait(&empty_bar[s], ph ^ 1u);
-      uint8_t* sK = smem + kTile128 + s * kStage;
+      uint8_t* sK = smem + L::kTile + s * kStage;
       mbar_expect_tx(&full_bar[s], kStage);
-      tma_load_4d(sK, &mapK, &full_bar[s], 0, h, j * 128, b);
-      tma_load_4d(sK + kTile128, &mapV, &full_bar[s], 0, h, j * 128, b);
+#pragma unroll
+      for (int pn = 0; pn < L::P; ++pn) {
+        tma_load_4d(sK + pn * kTile128, &mapK, &full_bar[s], 64 * pn, h, j * 128, b);
+        tma_load_4d(sK + L::kTile + pn * kTile128, &mapV, &full_bar[s], 64 * pn, h, j * 128, b);
+      }
       if (++s == kFwdStages) {
         s = 0;
         ph ^= 1u;
@@ -121,8 +171,8 @@ attn_wgmma_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
   const uint32_t s0 = smem_u32(smem);
   const uint64_t descQ = wgmma_desc(s0 + kTile64 * cw, 16, 1024);
-  const uint64_t descK = wgmma_desc(s0 + kTile128, 16, 1024);
-  const uint64_t descV = wgmma_desc(s0 + 2 * kTile128, kTile64, 1024);   // MN-major: a k-step is 16 rows of 128 B
+  const uint64_t descK = wgmma_desc(s0 + L::kTile, 16, 1024);
+  const uint64_t descV = wgmma_desc(s0 + 2 * L::kTile, L::kLboV, 1024);   // MN-major: a k-step is 16 rows of 128 B
   const float sl2 = a.scale * kLog2e;
   float s[64], o[NO / 2];
   uint32_t p[32];
@@ -133,7 +183,7 @@ attn_wgmma_fwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
   auto issue_qk = [&](int st) {
     const uint64_t dk = descK + (uint64_t)(st * (kStage >> 4));
 #pragma unroll
-    for (int k = 0; k < KS; ++k) Wgmma<128, 0, 0>::mma(s, descQ + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k > 0);
+    for (int k = 0; k < KS; ++k) Wgmma<128, 0, 0>::mma(s, descQ + kstep(k, kTile128), dk + kstep(k, kTile128), k > 0);
     wgmma_commit();
   };
 
@@ -218,15 +268,10 @@ __global__ void __launch_bounds__(kWgThreads, 1)
 attn_wgmma_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                       const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapdO,
                       const __grid_constant__ CUtensorMap mapdQ, const AttnArgs a) {
-  constexpr int KS = (DH + 15) / 16, NO = DH, BQ = 64;
-  constexpr uint32_t kStage = 2 * kTile64;                 // Q, dO
-  constexpr uint32_t kOffQ = 2 * kTile128;                 // after K, V
-  constexpr uint32_t kOffdS = kOffQ + kBwdStages * kStage; // [2][128 keys][64 queries] bf16
-  constexpr uint32_t kOffdQ = kOffdS + 2 * kTile128;       // [2][64 queries][DH] fp32
-  constexpr uint32_t kdQBytes = BQ * DH * 4;
-  constexpr uint32_t kOffL = kOffdQ + 2 * kdQBytes;        // [stages][64] LSE, [stages][64] D
-  constexpr uint32_t kOffBar = kOffL + kBwdStages * 2 * BQ * 4;
-  static_assert(kOffdQ % 128 == 0 && kdQBytes % 128 == 0 && kOffL % 16 == 0 && kOffBar % 8 == 0, "smem layout");
+  using L = BwdSmem<DH>;
+  constexpr int KS = (DH + 15) / 16, NO = DH, BQ = L::BQ, kBwdStages = L::kStages;
+  constexpr uint32_t kStage = L::kStage, kOffQ = L::kOffQ, kOffdS = L::kOffdS, kOffdQ = L::kOffdQ;
+  constexpr uint32_t kdQBytes = L::kdQBytes, kOffL = L::kOffL, kOffBar = L::kOffBar;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   float* sL = reinterpret_cast<float*>(smem + kOffL);
@@ -268,20 +313,26 @@ attn_wgmma_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
       mbar_wait(&empty_bar[s], ((uint32_t)(i / kBwdStages) & 1u) ^ 1u);
       uint8_t* sQ = smem + kOffQ + s * kStage;
       mbar_expect_tx(&full_bar[s], kStage + 2 * BQ * 4);
-      tma_load_4d(sQ, &mapQ, &full_bar[s], 0, h, i * BQ, b);
-      tma_load_4d(sQ + kTile64, &mapdO, &full_bar[s], 0, h, i * BQ, b);
+#pragma unroll
+      for (int pn = 0; pn < L::P; ++pn) {
+        tma_load_4d(sQ + pn * kTile64, &mapQ, &full_bar[s], 64 * pn, h, i * BQ, b);
+        tma_load_4d(sQ + L::kQ + pn * kTile64, &mapdO, &full_bar[s], 64 * pn, h, i * BQ, b);
+      }
       bulk_load_1d(sL + s * 2 * BQ, a.LSE + bh * a.N + i * BQ, BQ * 4, &full_bar[s]);
       bulk_load_1d(sL + s * 2 * BQ + BQ, a.Dv + bh * a.N + i * BQ, BQ * 4, &full_bar[s]);
     };
     if (threadIdx.x == 0) {
-      mbar_expect_tx(kv_bar, 2 * kTile128);
-      tma_load_4d(smem, &mapK, kv_bar, 0, h, k0, b);
-      tma_load_4d(smem + kTile128, &mapV, kv_bar, 0, h, k0, b);
+      mbar_expect_tx(kv_bar, 2 * L::kKV);
+#pragma unroll
+      for (int pn = 0; pn < L::P; ++pn) {
+        tma_load_4d(smem + pn * kTile128, &mapK, kv_bar, 64 * pn, h, k0, b);
+        tma_load_4d(smem + L::kKV + pn * kTile128, &mapV, kv_bar, 64 * pn, h, k0, b);
+      }
       for (int i = 0; i < kBwdStages - 1 && i < nq; ++i) load_block(i);
     }
     __syncwarp();
     const uint64_t descS = wgmma_desc(s0 + kOffdS, kTile64, 1024);   // A, MN-major: rows are keys, 64 queries wide
-    const uint64_t descK = wgmma_desc(s0, kTile64, 1024);            // B, MN-major: rows are keys, head dim wide
+    const uint64_t descK = wgmma_desc(s0, L::kLboK, 1024);           // B, MN-major: rows are keys, head dim wide
     mbar_wait(kv_bar, 0);
     float dq[NO / 2];
     for (int i = 0; i < nq; ++i) {
@@ -325,7 +376,7 @@ attn_wgmma_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
   setmaxnreg_inc<216>();
   const int cw = wg - 1;
   const uint64_t descKa = wgmma_desc(s0 + kTile64 * cw, 16, 1024);              // A of Sᵀ: this warpgroup's K rows
-  const uint64_t descVa = wgmma_desc(s0 + kTile128 + kTile64 * cw, 16, 1024);   // A of dPᵀ
+  const uint64_t descVa = wgmma_desc(s0 + L::kKV + kTile64 * cw, 16, 1024);     // A of dPᵀ
   const uint64_t descQk = wgmma_desc(s0 + kOffQ, 16, 1024);                     // B of Sᵀ (K-major Q block)
   const uint64_t descQm = wgmma_desc(s0 + kOffQ, kTile64, 1024);                // B of dK (the same tile, MN-major)
   const float sl2 = a.scale * kLog2e;
@@ -344,11 +395,11 @@ attn_wgmma_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < KS; ++k)
-      Wgmma<64, 0, 0>::mma(st, descKa + (uint64_t)(2 * k), descQk + so + (uint64_t)(2 * k), k > 0);
+      Wgmma<64, 0, 0>::mma(st, descKa + kstep(k, kTile128), descQk + so + kstep(k, kTile64), k > 0);
     wgmma_commit();
 #pragma unroll
     for (int k = 0; k < KS; ++k)
-      Wgmma<64, 0, 0>::mma(dpt, descVa + (uint64_t)(2 * k), descQk + so + (uint64_t)((kTile64 >> 4) + 2 * k), k > 0);
+      Wgmma<64, 0, 0>::mma(dpt, descVa + kstep(k, kTile128), descQk + so + (L::kQ >> 4) + kstep(k, kTile64), k > 0);
     wgmma_commit();
     const float* l_s = sL + s * 2 * BQ + 2 * (lane & 3);
     wgmma_wait<1>();   // Sᵀ; the exponentials run under dPᵀ
@@ -389,7 +440,7 @@ attn_wgmma_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
     wgmma_fence();
 #pragma unroll
     for (int kq = 0; kq < 4; ++kq)
-      WgmmaRS<NO, 1>::mma(dv, pp + 4 * kq, descQm + so + (uint64_t)((kTile64 >> 4) + kq * (2048 >> 4)), 1);
+      WgmmaRS<NO, 1>::mma(dv, pp + 4 * kq, descQm + so + (uint64_t)((L::kQ >> 4) + kq * (2048 >> 4)), 1);
 #pragma unroll
     for (int kq = 0; kq < 4; ++kq) WgmmaRS<NO, 1>::mma(dk, ps + 4 * kq, descQm + so + (uint64_t)(kq * (2048 >> 4)), 1);
     wgmma_commit();
@@ -416,8 +467,17 @@ attn_wgmma_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
 // =============================================================================================
 // Host
 // =============================================================================================
-bool attn_wgmma_shape_ok(int N, int M, int dh) {
-  return dh == 40 && N >= 512 && M >= 512 && N % 128 == 0 && M % 128 == 0;
+bool attn_wgmma_shape_ok(int B, int H, int N, int M, int dh) {
+  if (!(dh == 40 || dh == 80) || N < 512 || M < 512 || N % 128 != 0 || M % 128 != 0) return false;
+  if (dh == 40) return true;
+  // dh = 80: the wgmma kernels measured faster than mma.sync at every grid down to 64 CTAs (level 1 at B = 1), so the
+  // boundary is not a speed one: grids below half the SM count (that one included, on 132 SMs) keep the mma.sync
+  // kernels, and with them a level-1 shape on which those kernels stay checked against the switch
+  int sms = 0, dev = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (sms <= 0) sms = 132;
+  return 2LL * (N / 128) * H * B >= sms;
 }
 
 // TMA needs 16-byte aligned bases and strides; the library's callers always pass them, a caller that does not gets
@@ -437,8 +497,8 @@ int attn_wgmma_fwd(const AttnArgs& a, cudaStream_t st) {
   if (int e = head_map(&mK, a.K, a, a.M, a.ldk, a.k_bs, 128)) return e;
   if (int e = head_map(&mV, a.V, a, a.M, a.ldv, a.v_bs, 128)) return e;
   E4T_CHECK(a.ldo % 2 == 0 && a.o_bs % 2 == 0, "attention (wgmma): output strides must be even");
-  const size_t smem = 1024 + kTile128 + kFwdStages * 2 * kTile128 + 64;
-  auto kernel = attn_wgmma_fwd_kernel<40>;
+  const size_t smem = a.dh == 40 ? FwdSmem<40>::bytes : FwdSmem<80>::bytes;
+  auto kernel = a.dh == 40 ? attn_wgmma_fwd_kernel<40> : attn_wgmma_fwd_kernel<80>;
   E4T_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<dim3(a.N / 128, a.H, a.B), kWgThreads, smem, st>>>(mQ, mK, mV, a);
   E4T_COUNT_LAUNCH();
@@ -463,9 +523,8 @@ int attn_wgmma_bwd(const AttnArgs& a, cudaStream_t st) {
   }
   E4T_CHECK(a.lddk % 2 == 0 && a.dk_bs % 2 == 0 && a.lddv % 2 == 0 && a.dv_bs % 2 == 0,
             "attention (wgmma): gradient strides must be even");
-  const size_t smem = 1024 + 2 * kTile128 + kBwdStages * 2 * kTile64 + 2 * kTile128 + 2 * 64 * 40 * 4 +
-                      kBwdStages * 2 * 64 * 4 + 128;
-  auto kernel = attn_wgmma_bwd_kernel<40>;
+  const size_t smem = a.dh == 40 ? BwdSmem<40>::bytes : BwdSmem<80>::bytes;
+  auto kernel = a.dh == 40 ? attn_wgmma_bwd_kernel<40> : attn_wgmma_bwd_kernel<80>;
   E4T_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<dim3(a.M / 128, a.H, a.B), kWgThreads, smem, st>>>(mQ, mK, mV, mdO, mdQ, a);
   E4T_COUNT_LAUNCH();

@@ -346,8 +346,9 @@ def _bs(t):
 def attn_fwd(q, k, v, heads, scale=None):
     """q (B,N,H*dh), k/v (B,M,H*dh) bf16 (last dim contiguous; may be column slices of a fused projection).
     Returns (o (B,N,H*dh) bf16, lse (B,H,N) fp32).
-    dh == 40 with N and M multiples of 128, >= 512 (the 4096-token self-attention) runs the warpgroup (wgmma + TMA)
-    kernel; every other shape, or E4T_ATTN_WGMMA=0, the mma.sync kernel."""
+    dh == 40 or 80 with N and M multiples of 128, >= 512 (the 4096-token and 1024-token self-attention; for dh == 80
+    only grids of at least half as many 128-query CTAs as SMs) runs the warpgroup (wgmma + TMA) kernel; every other shape, or
+    E4T_ATTN_WGMMA=0, the mma.sync kernel."""
     assert q.dtype == BF16 and k.dtype == BF16 and v.dtype == BF16
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1
     Bn, N, C = q.shape
@@ -366,8 +367,8 @@ def attn_bwd(q, k, v, o, do, lse, heads, scale=None, dq=None, dk=None, dv=None, 
     """dq/dk/dv may be preallocated (e.g. column slices of one fused (B,N,3C) gradient buffer).
     fused=True: single-pass backward (S/dP computed once per tile pair, dQ reduced in fp32) when dh <= 80 and N >= 128;
     otherwise / fused=False the two-kernel (dK/dV, dQ) path.  The single-pass backward of a non-causal call with
-    dh == 40 and N, M multiples of 128, >= 512 runs the warpgroup (wgmma + TMA) kernel, which reduces dQ with bulk
-    tensor adds instead of scalar atomics; every other shape, or E4T_ATTN_WGMMA=0, the mma.sync kernel.
+    the shapes attn_fwd gives to the warpgroup kernels runs the warpgroup (wgmma + TMA) kernel, which reduces dQ with
+    bulk tensor adds instead of scalar atomics; every other shape, or E4T_ATTN_WGMMA=0, the mma.sync kernel.
     causal=True (N == M, dh <= 80): key j contributes to query i only if j <= i; o / lse must come from a forward that
     applied the same mask (attn_small_fwd)."""
     assert do.dtype == BF16 and do.stride(-1) == 1
