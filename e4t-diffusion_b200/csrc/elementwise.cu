@@ -141,6 +141,79 @@ extern "C" int e4t_resample2x(const void* x, void* y, int B, int H, int W, int C
 }
 
 // ---------------------------------------------------------------------------------------------
+// Resampling to explicit sizes on NHWC bf16 (C % 8 == 0); x is (B,Hx,Wx,C), y is (B,Hy,Wy,C)
+//   mode 0: nearest resize, torch's rule per axis (F.interpolate(size=..., mode="nearest")):
+//           src = min(floorf(dst * ((float)in / out)), in - 1)
+//   mode 1: its adjoint: x is the gradient at the resized size (Hx,Wx), y at the source size (Hy,Wy); each source
+//           pixel sums, in fp32 and in a fixed order, the resized pixels that map to it (one contiguous range per
+//           axis because the rule is monotone).  Gather form: no atomics, deterministic.
+//   mode 2: zero insertion to an explicit size (the adjoint of the stride-2 pick of a pad-1 stride-2 convolution,
+//           whose input (Hy,Wy) may be odd): y[2i][2j] = x[i][j], zero elsewhere; Hx = ceil(Hy/2), Wx = ceil(Wy/2).
+// One thread per 8 channels of one output pixel; the grid depends on the shapes only.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ int nearest_src(int dst, float scale, int in) {
+  return min((int)floorf((float)dst * scale), in - 1);
+}
+// first index j of the resized axis (length out) whose source index is >= i: the start of source pixel i's range
+__device__ __forceinline__ int nearest_first_dst(int i, float scale, int in, int out) {
+  int j = min(out, max(0, (int)ceilf((float)i / scale)));
+  while (j > 0 && nearest_src(j - 1, scale, in) >= i) --j;
+  while (j < out && nearest_src(j, scale, in) < i) ++j;
+  return j;
+}
+__global__ void resize_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, int B, int Hx, int Wx, int Hy, int Wy,
+                              int C, int mode) {
+  const int vpc = C / 8;
+  const long n = (long)B * Hy * Wy * vpc;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int cv = (int)(i % vpc);
+    long p = i / vpc;
+    const int ow = (int)(p % Wy);
+    p /= Wy;
+    const int oh = (int)(p % Hy);
+    const int b = (int)(p / Hy);
+    uint4 o;
+    if (mode == 0) {
+      const int sh = nearest_src(oh, (float)Hx / Hy, Hx), sw = nearest_src(ow, (float)Wx / Wy, Wx);
+      o = *reinterpret_cast<const uint4*>(x + (((long)b * Hx + sh) * Wx + sw) * C + cv * 8);
+    } else if (mode == 2) {
+      if ((oh & 1) == 0 && (ow & 1) == 0)
+        o = *reinterpret_cast<const uint4*>(x + (((long)b * Hx + oh / 2) * Wx + ow / 2) * C + cv * 8);
+      else
+        o = make_uint4(0, 0, 0, 0);
+    } else {
+      const float sh = (float)Hy / Hx, sw = (float)Wy / Wx;
+      const int h0 = nearest_first_dst(oh, sh, Hy, Hx), h1 = nearest_first_dst(oh + 1, sh, Hy, Hx);
+      const int w0 = nearest_first_dst(ow, sw, Wy, Wx), w1 = nearest_first_dst(ow + 1, sw, Wy, Wx);
+      float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      for (int hh = h0; hh < h1; ++hh)
+        for (int ww = w0; ww < w1; ++ww) {
+          const uint4 u = *reinterpret_cast<const uint4*>(x + (((long)b * Hx + hh) * Wx + ww) * C + cv * 8);
+          const float2 a = unpack_bf16(u.x), bb = unpack_bf16(u.y), c = unpack_bf16(u.z), d = unpack_bf16(u.w);
+          acc[0] += a.x; acc[1] += a.y; acc[2] += bb.x; acc[3] += bb.y;
+          acc[4] += c.x; acc[5] += c.y; acc[6] += d.x; acc[7] += d.y;
+        }
+      o = make_uint4(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]), pack_bf16(acc[4], acc[5]),
+                     pack_bf16(acc[6], acc[7]));
+    }
+    *reinterpret_cast<uint4*>(y + i * 8) = o;
+  }
+}
+extern "C" int e4t_resize_nearest(const void* x, void* y, int B, int Hx, int Wx, int Hy, int Wy, int C, int mode,
+                                  void* stream_) {
+  E4T_CHECK(B > 0 && Hx > 0 && Wx > 0 && Hy > 0 && Wy > 0 && C > 0 && C % 8 == 0 && mode >= 0 && mode <= 2,
+            "e4t_resize_nearest: bad args B=%d x %dx%d y %dx%d C=%d mode=%d", B, Hx, Wx, Hy, Wy, C, mode);
+  E4T_CHECK(mode != 2 || (Hx == (Hy + 1) / 2 && Wx == (Wy + 1) / 2),
+            "e4t_resize_nearest: zero insertion of %dx%d to %dx%d", Hx, Wx, Hy, Wy);
+  const long n = (long)B * Hy * Wy * (C / 8);
+  resize_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream_>>>((const bf16*)x, (bf16*)y, B, Hx, Wx, Hy, Wy, C,
+                                                                     mode);
+  E4T_COUNT_LAUNCH();
+  E4T_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
 // WeightOffsets, closed form (R = row_dim = in_features, C = column_dim = out_features)
 //   vx = w1 v + β1 (R)   vy = w2 v + β2 (C)   a = Wc vx (R)   b = Wr vy (C)   s = Wr 1 (C)
 // One warp per output row; rows [0,R) produce a (and vx), rows [R,R+C) produce b, s (and vy).
@@ -418,11 +491,13 @@ extern "C" int e4t_meanpool_bwd(const float* dout, void* dx, int B, int HW, int 
 // ---------------------------------------------------------------------------------------------
 // conv_in: NCHW fp32 (B,Cin<=8,H,W) -> NHWC bf16 (B,H,W,Cout), 3x3 pad 1.  w fp32 [Cout][Cin][3][3].
 // ---------------------------------------------------------------------------------------------
+// PARTIAL (W % 8 != 0): the last strip of each row is partial; its pixels past W read zeros and are not stored.
+template <bool PARTIAL>
 __global__ void conv_in_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
                                bf16* __restrict__ y, int B, int Cin, int H, int W, int Cout) {
   // one CTA per (b, h, 8-pixel strip); threads over Cout
   extern __shared__ float cin_sm[];  // [Cin][3][10] input patch
-  const int strips = W / 8;
+  const int strips = PARTIAL ? (W + 7) / 8 : W / 8;
   const int w0 = (blockIdx.x % strips) * 8;
   const int h = (blockIdx.x / strips) % H;
   const int b = blockIdx.x / (strips * H);
@@ -447,14 +522,19 @@ __global__ void conv_in_kernel(const float* __restrict__ x, const float* __restr
           for (int p = 0; p < 8; ++p) acc[p] += wv * cin_sm[ci * 30 + ky * 10 + p + kx];
         }
 #pragma unroll
-    for (int p = 0; p < 8; ++p) y[(((long)b * H + h) * W + w0 + p) * Cout + co] = __float2bfloat16(acc[p]);
+    for (int p = 0; p < 8; ++p)
+      if (!PARTIAL || w0 + p < W) y[(((long)b * H + h) * W + w0 + p) * Cout + co] = __float2bfloat16(acc[p]);
   }
 }
 extern "C" int e4t_conv_in_fwd(const float* x, const float* w, const float* bias, void* y, int B, int Cin, int H,
                                int W, int Cout, void* stream_) {
-  E4T_CHECK(W % 8 == 0 && Cin <= 16, "e4t_conv_in_fwd: W %% 8 != 0 or Cin > 16");
-  conv_in_kernel<<<B * H * (W / 8), 128, (size_t)Cin * 30 * sizeof(float), (cudaStream_t)stream_>>>(x, w, bias, (bf16*)y,
-                                                                                                   B, Cin, H, W, Cout);
+  E4T_CHECK(B > 0 && H > 0 && W > 0 && Cin <= 16, "e4t_conv_in_fwd: bad image %dx%dx%d or Cin %d > 16", B, H, W, Cin);
+  const size_t smem = (size_t)Cin * 30 * sizeof(float);
+  if (W % 8 == 0)
+    conv_in_kernel<false><<<B * H * (W / 8), 128, smem, (cudaStream_t)stream_>>>(x, w, bias, (bf16*)y, B, Cin, H, W, Cout);
+  else
+    conv_in_kernel<true><<<B * H * ((W + 7) / 8), 128, smem, (cudaStream_t)stream_>>>(x, w, bias, (bf16*)y, B, Cin, H,
+                                                                                        W, Cout);
   E4T_COUNT_LAUNCH();
   E4T_LAUNCH_CHECK();
   return 0;

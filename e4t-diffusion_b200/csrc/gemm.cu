@@ -616,7 +616,8 @@ extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int
   return launch_gemm(mA, mB, g, stream);
 }
 
-// x: NHWC bf16 [B][Hin][Win][Cin];  w: bf16 [9][Cout][Cin] (tap = ky*3+kx);  out: [B*H*W][Cout] (NHWC), H = Hin/stride.
+// x: NHWC bf16 [B][Hin][Win][Cin];  w: bf16 [9][Cout][Cin] (tap = ky*3+kx);  out: [B*H*W][Cout] (NHWC),
+// H = ceil(Hin/stride).
 // bias fp32 [Cout]; rowgroup fp32 [B][Cout] (time-embedding projection) ; residual bf16 NHWC.
 // Padding: pad_lo zero rows / columns on the top and left (1 = the symmetric pad-1 convolution); the taps of output
 // pixel (y, x) read input (stride*y + ky - pad_lo, stride*x + kx - pad_lo), and whatever falls outside the input, on
@@ -633,6 +634,9 @@ extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int
 // last tap-(0, 0) position, stride*(out - 1) - pad_lo, so each image yields exactly H x W output pixels; the tap's
 // (dx, dy) are the load's im2col offsets.  The shared-memory tile is byte-identical to the tiled box's (128 rows of 64
 // channels, SWIZZLE_128B), so the MMA warpgroups and the epilogue do not know which load filled it.
+// Odd input sides (stride 2, pad 1 only) give ceil(Hin/2) outputs and always take the im2col load: its upper corner
+// 2*(H - 1) - 1 - (Hin - 1) is -1 for an odd side (-2 for an even one), and the last output's taps read the bottom /
+// right pad as out-of-bounds zeros.
 static bool conv_tiled_fits(int H, int W) {
   if (W > 128) return W % 128 == 0;
   if (128 % W) return false;
@@ -644,9 +648,10 @@ static int conv3x3_impl(const void* x, const void* w, void* out, int B, int Hin,
                         int force_bn, bool im2col, cudaStream_t stream) {
   E4T_CHECK(B > 0 && Hin > 0 && Win > 0 && Cout > 0, "e4t_conv3x3: bad dims B=%d H=%d W=%d Cout=%d", B, Hin, Win, Cout);
   E4T_CHECK(Cin % 64 == 0, "e4t_conv3x3: Cin must be a multiple of 64 (got %d)", Cin);
-  E4T_CHECK(stride == 1 || (stride == 2 && Hin % 2 == 0 && Win % 2 == 0), "e4t_conv3x3: bad stride/size");
+  E4T_CHECK(stride == 1 || (stride == 2 && ((Hin % 2 == 0 && Win % 2 == 0) || (pad_lo == 1 && im2col))),
+            "e4t_conv3x3: bad stride/size");
   E4T_CHECK(pad_lo == 1 || (stride == 2 && pad_lo == 0), "e4t_conv3x3: bad padding %d for stride %d", pad_lo, stride);
-  const int H = Hin / stride, W = Win / stride;
+  const int H = (Hin + stride - 1) / stride, W = (Win + stride - 1) / stride;
   const bool wide = W > 128;
   const int img = H * W;
   int BH = 1, BB = 1;
@@ -721,11 +726,13 @@ extern "C" int e4t_conv3x3_im2col_bf16(const void* x, const void* w, void* out, 
 }
 
 // 3x3 / stride 2 / pad 1 (diffusers Downsample2D.conv, e4t/models/unet_2d_blocks.py:801-808): x [B][H][W][Cin] ->
-// out [B][H/2][W/2][Cout].  The tiled box where it covers the output size, im2col elsewhere.
+// out [B][ceil(H/2)][ceil(W/2)][Cout].  Even sizes: the tiled box where it covers the output size, im2col elsewhere;
+// odd sizes: im2col.
 extern "C" int e4t_conv3x3_s2_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                                    const float* bias, int force_bn, void* stream_) {
+  const bool odd = (H % 2) != 0 || (W % 2) != 0;
   return conv3x3_impl(x, w, out, B, H, W, Cin, Cout, 2, 1, 0, bias, nullptr, nullptr, force_bn,
-                      !conv_tiled_fits(H / 2, W / 2), (cudaStream_t)stream_);
+                      odd || !conv_tiled_fits(H / 2, W / 2), (cudaStream_t)stream_);
 }
 
 // 3x3 / stride 2 with pad_lo zero rows / columns on the top and left: pad_lo = 1 is e4t_conv3x3_s2_bf16; pad_lo = 0 is

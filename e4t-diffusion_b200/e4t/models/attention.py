@@ -132,11 +132,22 @@ class AttentionBlock(nn.Module):
         qkv = ops.gemm(h.view(B * N, C), w_qkv, bias=b_qkv).view(B, N, 3 * C)
         scale = 1.0 / math.sqrt(C / self.num_heads)
         o = torch.empty((B, N, C), device=x.device, dtype=torch.bfloat16)
-        chunk = max(1, ATTN_SCORE_BYTES // (N * N * 4))
+        # N % 8 != 0 (a latent with an odd side): the score and probability rows get a pitch of Np = N rounded up to 8
+        # elements, which TMA and the softmax's vector loads need.  The pad columns of the scores are set to -inf after
+        # the GEMM (whose TMA epilogue may write zeros up to the next 16-byte boundary past N), so their probabilities
+        # are exact zeros; P·V reads K = N columns of P (its K tail is TMA out-of-bounds zero fill)
+        Np = (N + 7) // 8 * 8
+        chunk = max(1, ATTN_SCORE_BYTES // (N * Np * 4))
         for i in range(0, B, chunk):
             q, k, v = qkv[i:i + chunk, :, :C], qkv[i:i + chunk, :, C:2 * C], qkv[i:i + chunk, :, 2 * C:]
-            s = ops.gemm(q, k, alpha=scale, out_dtype=torch.float32)               # (b, N, N) fp32
-            p = ops.softmax_rows(s)
+            if Np == N:
+                s = ops.gemm(q, k, alpha=scale, out_dtype=torch.float32)           # (b, N, N) fp32
+                p = ops.softmax_rows(s)
+            else:
+                s = torch.empty((q.shape[0], N, Np), device=x.device, dtype=torch.float32)
+                ops.gemm(q, k, alpha=scale, out=s[..., :N])
+                s[..., N:] = float("-inf")
+                p = ops.softmax_rows(s)[..., :N]
             del s
             ops.gemm(p, v, b_mn=True, out=o[i:i + chunk])
         w_o = FN.prepared(self.proj_attn.weight, "bf16", lambda t: t.to(torch.bfloat16).contiguous())

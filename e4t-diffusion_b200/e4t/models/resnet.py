@@ -47,10 +47,12 @@ class Upsample2D(nn.Module):
             self.Conv2d_0 = conv
 
     def forward(self, hidden_states, output_size=None):
-        if output_size is not None:
-            raise NotImplementedError("output_size forwarding (non power-of-two latents) is not supported")
+        """hidden_states (B,H,W,C); output_size: the (height, width) to resize to instead of (2H, 2W) — the skip
+        connection's size, forwarded by the UNet when a latent side is not a multiple of its up-sampling factor."""
         conv = self.conv if self.name == "conv" else self.Conv2d_0
-        return conv3x3(conv, FN.ResampleFn.apply(hidden_states, 0))
+        if output_size is None:
+            return conv3x3(conv, FN.ResampleFn.apply(hidden_states, 0))
+        return conv3x3(conv, FN.ResizeNearestFn.apply(hidden_states, tuple(output_size)))
 
 
 class Downsample2D(nn.Module):

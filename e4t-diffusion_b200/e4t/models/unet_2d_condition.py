@@ -163,8 +163,26 @@ class UNet2DConditionModel(ModelMixin, ConfigMixin):
     def latent_multiple(self) -> int:
         """Latent heights and widths must be multiples of this: the overall down-sampling factor 2^(levels - 1) (8 for
         SD-v1.4, i.e. images in multiples of 64 px), so every stride-2 convolution sees an even size and each up block
-        meets its skip connections at their size."""
+        meets its skip connections at their size.  1 while enable_any_latent_size() is in effect."""
+        if getattr(self, "_any_latent_size", False):
+            return 1
         return 2 ** (len(self.config.block_out_channels) - 1)
+
+    @property
+    def min_latent_size(self) -> int:
+        """Smallest latent height and width the UNet takes: 2^(levels - 1), so the deepest level is at least 1 x 1."""
+        return 2 ** (len(self.config.block_out_channels) - 1)
+
+    def enable_any_latent_size(self):
+        """Accept any latent height and width of at least `min_latent_size` (images in multiples of the VAE's factor,
+        8 px for SD): stride-2 convolutions at odd sides give ceil(side / 2), and each up block resizes to its skip
+        connection's size, as diffusers does when it forwards the up-sampling size.  Sizes that are multiples of
+        2^(levels - 1) run exactly as with the switch off."""
+        self._any_latent_size = True
+
+    def disable_any_latent_size(self):
+        """Back to the default: latent sides must be multiples of 2^(levels - 1)."""
+        self._any_latent_size = False
 
     # ---- processor plumbing (unet_2d_condition.py:291-341) ---------------------------------------
     @property
@@ -251,8 +269,14 @@ class UNet2DConditionModel(ModelMixin, ConfigMixin):
         if attention_mask is not None or class_labels is not None or down_block_additional_residuals is not None \
                 or mid_block_additional_residual is not None:
             raise NotImplementedError("attention_mask / class_labels / ControlNet residuals are not on the E4T path")
-        if any(s % (2 ** self.num_upsamplers) != 0 for s in sample.shape[-2:]):
-            raise NotImplementedError("latent size must be a multiple of 2**num_upsamplers")
+        # upsample sizes are forwarded when a side is not a multiple of the overall up factor (:426-436)
+        forward_upsample_size = any(s % (2 ** self.num_upsamplers) != 0 for s in sample.shape[-2:])
+        if forward_upsample_size and not getattr(self, "_any_latent_size", False):
+            raise NotImplementedError("latent size must be a multiple of 2**num_upsamplers "
+                                      "(enable_any_latent_size() lifts this)")
+        if min(sample.shape[-2:]) < self.min_latent_size:
+            raise E4TError(f"latents of {sample.shape[-2]} x {sample.shape[-1]}: the sides must be at least "
+                           f"{self.min_latent_size}")
         if not torch.is_grad_enabled():
             FN.bump_nograd_fwd_epoch()      # no-grad forwards always rebuild W_eff from the current parameters
         if self.config.center_input_sample:
@@ -273,14 +297,17 @@ class UNet2DConditionModel(ModelMixin, ConfigMixin):
         if return_encoder_outputs:                                                 # :517-521
             res += (x,)
             return dict(down_block_samples=tuple(t.permute(0, 3, 1, 2) for t in res))
-        for blk in self.up_blocks:                                                 # :527-551
+        upsample_size = None
+        for i, blk in enumerate(self.up_blocks):                                   # :527-551
             n = len(blk.resnets)
             skips, res = res[-n:], res[:-n]
+            if i < len(self.up_blocks) - 1 and forward_upsample_size:
+                upsample_size = tuple(res[-1].shape[1:3])                          # NHWC: the next skip's (H, W)
             if getattr(blk, "has_cross_attention", False):
                 x = blk(hidden_states=x, temb=emb, res_hidden_states_tuple=skips, encoder_hidden_states=ehs,
-                        cross_attention_kwargs=cross_attention_kwargs)
+                        cross_attention_kwargs=cross_attention_kwargs, upsample_size=upsample_size)
             else:
-                x = blk(hidden_states=x, temb=emb, res_hidden_states_tuple=skips)
+                x = blk(hidden_states=x, temb=emb, res_hidden_states_tuple=skips, upsample_size=upsample_size)
         n = self.conv_norm_out
         x = FN.GroupNormFn.apply(x, n.weight, n.bias, n.num_groups, n.eps, True)  # :554-556
         out = FN.ConvOutFn.apply(x, self.conv_out.weight, self.conv_out.bias)       # :557 -> (B,4,H,W) fp32

@@ -165,6 +165,9 @@ class StableDiffusionE4TPipeline:
         if height % px or width % px:
             raise ValueError(f"height and width must be multiples of {px} px (the UNet's down-sampling factor "
                              f"{self.unet.latent_multiple} times the VAE's {self.vae_scale_factor}); got {height} x {width}")
+        px_min = self.unet.min_latent_size * self.vae_scale_factor
+        if min(height, width) < px_min:
+            raise ValueError(f"height and width must be at least {px_min} px; got {height} x {width}")
         assert negative_prompt is None, "negative_prompt is not supported"            # :153
         batch_size = 1 if isinstance(prompt, str) else len(prompt)
         device = self._execution_device

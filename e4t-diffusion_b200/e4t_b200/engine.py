@@ -258,6 +258,9 @@ class PretrainStep:
         if latents.shape[-2] % m or latents.shape[-1] % m:
             raise E4TError(f"latents of {latents.shape[-2]} x {latents.shape[-1]}: the sides must be multiples of the "
                            f"UNet's down-sampling factor {m}")
+        if min(latents.shape[-2:]) < self.unet.min_latent_size:
+            raise E4TError(f"latents of {latents.shape[-2]} x {latents.shape[-1]}: the sides must be at least "
+                           f"{self.unet.min_latent_size}")
         timesteps, input_ids = batch["timesteps"], batch["input_ids"]
         B = latents.shape[0]
         emb = self.text.get_input_embeddings()

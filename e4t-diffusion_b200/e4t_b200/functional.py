@@ -323,6 +323,7 @@ class Conv3x3S2Fn(torch.autograd.Function):
         y = ops.conv3x3_s2(x, w9, bias=bias)
         need_dw = wp is not None and ctx.needs_input_grad[4]
         ctx.save_for_backward(w9_dgrad, x if need_dw else None)
+        ctx.in_hw = tuple(x.shape[1:3])
         return y
 
     @staticmethod
@@ -330,7 +331,10 @@ class Conv3x3S2Fn(torch.autograd.Function):
         w9_dgrad, x = ctx.saved_tensors
         dy = _c(dy)
         Cout = dy.shape[-1]
-        up = ops.resample2x(dy, 3)                                              # zero insertion
+        if ctx.in_hw == (2 * dy.shape[1], 2 * dy.shape[2]):
+            up = ops.resample2x(dy, 3)                                          # zero insertion
+        else:
+            up = ops.zero_insert(dy, ctx.in_hw)                                 # to an odd input side
         dx = conv3x3_any(up, w9_dgrad) if ctx.needs_input_grad[0] else None
         db = dw = None
         if ctx.needs_input_grad[3]:
@@ -351,6 +355,23 @@ class ResampleFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         return ops.resample2x(_c(dy), 1 if ctx.mode == 0 else 3), None
+
+
+class ResizeNearestFn(torch.autograd.Function):
+    """Nearest resize of NHWC to an explicit size (diffusers Upsample2D with output_size); backward is the adjoint.
+    An exact 2x size runs the x2 kernel (ResampleFn's modes 0 / 1), so sizes that need no explicit size record no
+    new op."""
+
+    @staticmethod
+    def forward(ctx, x, size):
+        size = tuple(int(s) for s in size)
+        ctx.in_hw = tuple(x.shape[1:3])
+        ctx.x2 = size == (2 * x.shape[1], 2 * x.shape[2])
+        return ops.resample2x(_c(x), 0) if ctx.x2 else ops.resize_nearest(_c(x), size)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return (ops.resample2x(_c(dy), 1) if ctx.x2 else ops.resize_nearest_bwd(_c(dy), ctx.in_hw)), None
 
 
 class ConvOutFn(torch.autograd.Function):

@@ -114,13 +114,13 @@ def conv3x3_im2col(x, w9, *, bias=None, rowgroup=None, residual=None, out_dtype=
 
 
 def conv3x3_s2(x, w9, *, bias=None, force_bn=0, pad_lo=1):
-    """3x3 stride-2 convolution on NHWC bf16 (Downsample2D): (B,H,W,Cin) -> (B,H/2,W/2,Cout).
-    pad_lo=1: pad 1 on every side; pad_lo=0: one zero row / column on the bottom and right only (diffusers
-    Downsample2D(padding=0), the VAE encoder)."""
+    """3x3 stride-2 convolution on NHWC bf16 (Downsample2D): (B,H,W,Cin) -> (B,ceil(H/2),ceil(W/2),Cout).
+    pad_lo=1: pad 1 on every side (any H, W); pad_lo=0: one zero row / column on the bottom and right only (diffusers
+    Downsample2D(padding=0), the VAE encoder; H, W even)."""
     assert x.dtype == BF16 and w9.dtype == BF16 and x.is_contiguous() and w9.is_contiguous()
     Bn, H, W, Cin = x.shape
     Cout = w9.shape[1]
-    out = torch.empty((Bn, H // 2, W // 2, Cout), device=x.device, dtype=BF16)
+    out = torch.empty((Bn, (H + 1) // 2, (W + 1) // 2, Cout), device=x.device, dtype=BF16)
     if pad_lo == 1:
         _lib.call("e4t_conv3x3_s2_bf16", ptr(x), ptr(w9), ptr(out), c_int(Bn), c_int(H), c_int(W), c_int(Cin),
                   c_int(Cout), ptr(bias), c_int(force_bn), stream())
@@ -225,6 +225,37 @@ def resample2x(x, mode):
         H, W = Hx // 2, Wx // 2
         y = torch.empty((Bn, H, W, C), device=x.device, dtype=BF16)
     _lib.call("e4t_resample2x", ptr(x), ptr(y), c_int(Bn), c_int(H), c_int(W), c_int(C), c_int(mode), stream())
+    return y
+
+
+def _resize_args(x, size):
+    assert x.dtype == BF16 and x.is_contiguous() and x.dim() == 4
+    Bn, Hx, Wx, C = x.shape
+    Hy, Wy = (int(s) for s in size)
+    y = torch.empty((Bn, Hy, Wy, C), device=x.device, dtype=BF16)
+    return y, (ptr(x), ptr(y), c_int(Bn), c_int(Hx), c_int(Wx), c_int(Hy), c_int(Wy), c_int(C))
+
+
+def resize_nearest(x, size):
+    """Nearest resize of NHWC bf16 (B,Hi,Wi,C) to (B,*size,C) with torch's index rule: bit-identical to
+    F.interpolate(size=size, mode="nearest") (diffusers Upsample2D with output_size)."""
+    y, args = _resize_args(x, size)
+    _lib.call("e4t_resize_nearest", *args, c_int(0), stream())
+    return y
+
+
+def resize_nearest_bwd(dy, in_size):
+    """Adjoint of resize_nearest: dy (B,Ho,Wo,C) at the resized size -> (B,*in_size,C) (fp32 sums, deterministic)."""
+    dx, args = _resize_args(dy, in_size)
+    _lib.call("e4t_resize_nearest", *args, c_int(1), stream())
+    return dx
+
+
+def zero_insert(dy, size):
+    """Zero insertion of (B,Ho,Wo,C) to (B,*size,C), y[2i, 2j] = dy[i, j]: the adjoint of the stride-2 pick of a pad-1
+    stride-2 convolution whose input is `size` (either side may be odd; Ho = ceil(size[0] / 2))."""
+    y, args = _resize_args(dy, size)
+    _lib.call("e4t_resize_nearest", *args, c_int(2), stream())
     return y
 
 

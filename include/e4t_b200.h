@@ -51,13 +51,14 @@ int e4t_conv3x3_im2col_bf16(const void* x, const void* w, void* out, int B, int 
 
 /* 3x3 / stride 2 / pad 1 (diffusers Downsample2D.conv, built at e4t/models/unet_2d_blocks.py:801-808): computed at the
  * OUTPUT resolution — the implicit-GEMM A operand is gathered with TMA element strides.  x [B][H][W][Cin] ->
- * out [B][H/2][W/2][Cout], H and W even.  Output sizes outside e4t_conv3x3_bf16's tiled domain load in im2col mode. */
+ * out [B][ceil(H/2)][ceil(W/2)][Cout].  Output sizes outside e4t_conv3x3_bf16's tiled domain, and odd H or W, load in
+ * im2col mode. */
 int e4t_conv3x3_s2_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout,
                         const float* bias, int force_bn, void* stream);
 /* 3x3 / stride 2 with pad_lo zero rows / columns on the top and left (1 = e4t_conv3x3_s2_bf16; 0 = diffusers
  * Downsample2D(padding=0): `F.pad(x, (0, 1, 0, 1))` then an unpadded stride-2 conv, the VAE encoder's downsamplers built at
  * e4t/models/unet_2d_blocks.py:937-1000 (DownEncoderBlock2D)).  Taps read x[2y + ky - pad_lo][2x + kx - pad_lo]; rows
- * and columns outside the input are zero.  x [B][H][W][Cin] -> out [B][H/2][W/2][Cout]. */
+ * and columns outside the input are zero.  x [B][H][W][Cin] -> out [B][H/2][W/2][Cout]; pad_lo = 0 needs H and W even. */
 int e4t_conv3x3_s2p_bf16(const void* x, const void* w, void* out, int B, int H, int W, int Cin, int Cout, int pad_lo,
                          const float* bias, int force_bn, void* stream);
 /* Weight gradient of the 3x3 / stride 1 / pad 1 convolution: dw9[tap][co][ci] += sum dy[b][y][x][co] * x[b][y+ky-1][x+kx-1][ci]
@@ -162,7 +163,13 @@ int e4t_geglu_bwd(const void* h, const void* dout, void* dh, long long rows, int
 /* 2x spatial resampling on NHWC (H, W = the SMALL resolution): mode 0 nearest upsample (diffusers Upsample2D),
  * 1 its adjoint, 2 stride-2 pick (Downsample2D = stride-1 conv sampled at even positions), 3 zero insertion. */
 int e4t_resample2x(const void* x, void* y, int B, int H, int W, int C, int mode, void* stream);
-/* UNet conv_in (unet_2d_condition.py:481): NCHW fp32 -> NHWC bf16; w fp32 [Cout][Cin][3][3]. */
+/* Resampling to explicit sizes on NHWC bf16 (C % 8 == 0), x [B][Hx][Wx][C] -> y [B][Hy][Wy][C]: mode 0 nearest resize
+ * with torch's index rule, src = min(floorf(dst * ((float)in / out)), in - 1) per axis (diffusers Upsample2D with
+ * output_size, F.interpolate(size=..., mode="nearest")); 1 its adjoint (x at the resized size, y at the source size;
+ * fp32 sums in a fixed order, no atomics); 2 zero insertion y[2i][2j] = x[i][j] with Hx = ceil(Hy/2), Wx = ceil(Wy/2)
+ * (the adjoint of the pad-1 stride-2 pick at odd input sizes). */
+int e4t_resize_nearest(const void* x, void* y, int B, int Hx, int Wx, int Hy, int Wy, int C, int mode, void* stream);
+/* UNet conv_in (unet_2d_condition.py:481): NCHW fp32 -> NHWC bf16; w fp32 [Cout][Cin][3][3]; any W. */
 int e4t_conv_in_fwd(const float* x, const float* w, const float* bias, void* y, int B, int Cin, int H, int W,
                     int Cout, void* stream);
 /* UNet conv_out (unet_2d_condition.py:557): NHWC bf16 -> NCHW fp32, and its input gradient. */

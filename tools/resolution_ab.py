@@ -2,7 +2,7 @@
 oracle's composition on torch ops under bf16 autocast, channels_last 4-D weights and activations, cuDNN convolutions,
 SDPA attention).
 
-    python tools/resolution_ab.py [--iters 10] [--sizes 512x512,768x512,...] [--skip-conv]
+    python tools/resolution_ab.py [--iters 10] [--sizes 512x512,768x512,...] [--skip-conv] [--ragged]
 
 1. Per image size (H x W pixels): one SD-v1.4 classifier-free-guidance denoising step (encoder-half UNet on one
    latent, E4T encoder head with CLIP ViT-H/14, CLIP-L text encoder, full UNet on two latents) and the SD VAE decode of
@@ -11,6 +11,9 @@ SDPA attention).
    convolution shapes, where both accept the input.
 3. e4t_conv3x3_wgrad picks its load by shape, so its tiled load is timed at 512² training shapes (B = 16) and its
    im2col load on the same batch with every row one pixel shorter, compared per pixel.
+--ragged: sizes that are multiples of 8 px but not of 64 (520², 544 x 672, 504 x 776), each followed by the nearest
+multiple-of-64 size, with UNet2DConditionModel.enable_any_latent_size(): the difference is the cost of the im2col
+loads, the explicit-size resize and zero insertion, and the mma.sync attention at ragged token counts.
 The card, its power limit and SM clock are read in the same run.  Synthetic weights (PyTorch's default init)."""
 import argparse
 import os
@@ -25,9 +28,12 @@ for p in (ROOT, os.path.join(ROOT, "e4t-diffusion_b200")):
 import torch  # noqa: E402
 
 from oracle import e4t_oracle as O  # noqa: E402
+from oracle import ragged_oracle as RO  # noqa: E402
 from oracle import vae_oracle as V  # noqa: E402
 
 SIZES = "512x512,768x512,512x768,576x576,640x640,768x768"
+# each ragged size, then its nearest multiple-of-64 size (ties round down)
+RAGGED = "520x520,512x512,544x672,512x640,504x776,512x768"
 
 
 def card():
@@ -80,12 +86,12 @@ def e4t_cfg_step(unet, enc, text, lat, pix, ids, idx, t, ehs_e4t, class_embed):
 def torch_cfg_step(sd_u, sd_e, sd_t, lat, pix, ids, idx, t, ehs_e4t, class_embed):
     tok = sd_t["text_model.embeddings.token_embedding.weight"]
     with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
-        e = O.unet_forward(sd_u, O.SD14_UNET, lat, t, ehs_e4t, return_encoder_outputs=True)
+        e = RO.unet_forward(sd_u, O.SD14_UNET, lat, t, ehs_e4t, return_encoder_outputs=True)
         dom = class_embed + 0.1 * O.encoder_forward(sd_e, O.VIT_H14, pix, e["down_block_samples"]).float()
         emb = tok[ids].clone()
         emb[:, idx, :] = dom.to(emb.dtype)
         ehs = O.text_forward(sd_t, O.CLIP_TEXT_L, inputs_embeds=emb)
-        pred = O.unet_forward(sd_u, O.SD14_UNET, torch.cat([lat, lat]), t.expand(2), torch.cat([ehs_e4t, ehs]))
+        pred = RO.unet_forward(sd_u, O.SD14_UNET, torch.cat([lat, lat]), t.expand(2), torch.cat([ehs_e4t, ehs]))
         u, c = pred.float().chunk(2)
         return u + 7.5 * (c - u)
 
@@ -129,12 +135,17 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--sizes", default=SIZES)
     ap.add_argument("--skip-conv", action="store_true")
+    ap.add_argument("--ragged", action="store_true", help=f"time {RAGGED} (sizes that are multiples of 8 px)")
     args = ap.parse_args()
+    if args.ragged:
+        args.sizes = RAGGED
     print("card:", card())
     import bench
     from e4t.models.autoencoder_kl import AutoencoderKL
     torch.backends.cudnn.benchmark = True
     unet, enc, text = bench.build_models("cuda")
+    if args.ragged:
+        unet.enable_any_latent_size()
     sd_u, sd_e, sd_t = (cl({k: v for k, v in m.state_dict().items()}) for m in (unet, enc, text))
     sd_t = {k: v.float() for k, v in sd_t.items()}
     b = bench.to_device(bench.host_batch(1, 3, pinned=False), "cuda")
