@@ -55,6 +55,15 @@ class WOBank:
     def __init__(self, attn_modules):
         self.modules = list(attn_modules)
         assert self.modules
+        # the kernels read W, a, bc, vx, vy and the .grad rows as float4 (W_eff stores as 4 bf16) at offsets that are
+        # multiples of R or C, and the projection GEMMs need leading dimensions R and C that are multiples of 8
+        for i, m in enumerate(self.modules):
+            for name in ("to_q", "to_k", "to_v"):
+                lin = getattr(m, name)
+                if lin.in_features % 8 or lin.out_features % 8:
+                    raise ValueError(f"WOBank: attention module {i} ({type(m).__name__}), {name}: {lin.in_features} "
+                                     f"in- and {lin.out_features} out-features; the WeightOffsets bank needs both to "
+                                     f"be multiples of 8")
         self.device = self.modules[0].to_q.weight.device
         self.groups = []      # (module, group name, [(linear, wo), ...])
         for m in self.modules:

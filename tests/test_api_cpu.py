@@ -113,6 +113,22 @@ def test_wo_bank_record_layout_matches_library():
     assert lib.e4t_wo_bank_record_size() == ctypes.sizeof(_WOProj) == 23 * 8 + 8
 
 
+@pytest.mark.parametrize("query_dim,cross_dim,heads,dim_head,bad", [
+    (64, 30, 4, 16, "to_k: 30 in-"),         # kv in-features not a multiple of 8
+    (36, None, 4, 16, "to_q: 36 in-"),       # self-attention, query_dim 36 (a multiple of 4, not of 8)
+    (64, 96, 3, 4, "to_q: 64 in- and 12 out-"),  # inner dim 12
+])
+def test_wo_bank_refuses_sides_that_are_not_multiples_of_8(query_dim, cross_dim, heads, dim_head, bad):
+    """The bank's vector loads and the projection GEMMs need R and C to be multiples of 8: WOBank refuses other shapes
+    when it is built, before it allocates anything or calls the library (so this runs on the CPU)."""
+    from e4t.models.cross_attention import CrossAttention
+    from e4t_b200.wobank import WOBank
+    ok = CrossAttention(query_dim=64, cross_attention_dim=768, heads=8, dim_head=8)
+    badm = CrossAttention(query_dim=query_dim, cross_attention_dim=cross_dim, heads=heads, dim_head=dim_head)
+    with pytest.raises(ValueError, match=r"attention module 1 \(CrossAttention\), " + re.escape(bad)):
+        WOBank([ok, badm])
+
+
 @pytest.mark.parametrize("R,C", [(8, 8), (24, 16), (40, 72)])
 def test_wo_closed_form_gradients_match_autograd(R, C):
     """SURVEY.md Appendix A backward identities (what wo_bank_*_kernel implement) vs autograd of the literal module."""

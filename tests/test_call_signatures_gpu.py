@@ -18,7 +18,7 @@ Per output: everything in the logical extent is finite, everything outside it is
 the reference RMS is within the bound the op's own kernel test uses, and every block of the kernel's tiling (128 x 64
 for the GEMM engine, (image, head, 64 queries) for attention, (image, group) for GroupNorm, rows for the row kernels)
 has an RMS error of at most 4x that bound (relative to the RMS of the whole reference), so one wrong tile cannot hide in
-a large tensor.  The WeightOffsets bank (_lib.call directly) is covered by test_e2e_gpu.py.
+a large tensor.  The WeightOffsets bank (_lib.call directly) is checked against fp64 by test_wo_bank_gpu.py.
 """
 import gc
 import inspect
