@@ -117,8 +117,12 @@ __device__ __forceinline__ void gemm_epilogue(const GemmArgs& g, const float* ac
 // RES_TMA (bf16 output only): the residual tile already sits in the staging buffer, loaded by gemm_residual_load into
 // the bytes each thread's outputs go to; the thread waits on res_bar, adds the bf16 pair it finds there in place of
 // the global read and overwrites it with the output.  The sum and its order are the same, so the output is too.
+// Alpha, bias and row-group addend are applied to the accumulators in place first, in loops without per-column
+// branches: a row's bias / row-group loads then issue together, where a branch per column pair made each wait for the
+// previous pair's load.  Columns past N add a clamped, in-bounds value (TMA clips them); __fmul_rn / __fadd_rn keep
+// every product and sum separately rounded, as in gemm_epilogue, so the outputs do not change.
 template <int BN, typename OutT, bool RES_TMA = false>
-__device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUtensorMap* mapO, const float* acc,
+__device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUtensorMap* mapO, float* acc,
                                                   uint8_t* stg, int m_t, int n0, int bz, int wg_row, uint32_t bar_id,
                                                   uint64_t* res_bar = nullptr, uint32_t res_ph = 0) {
   static_assert(!RES_TMA || sizeof(OutT) == 2, "the TMA-loaded residual fills a bf16 staging buffer");
@@ -130,6 +134,35 @@ __device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUten
   const int lane = tid & 31;
   const int w = tid >> 5;
   const int row0 = m_t * kBM + wg_row;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = row0 + w * 16 + (lane >> 2) + 8 * h;
+    if (m >= g.M) continue;
+    if (g.alpha != 1.f) {  // x * 1 is x
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        acc[4 * j + 2 * h] = __fmul_rn(acc[4 * j + 2 * h], g.alpha);
+        acc[4 * j + 2 * h + 1] = __fmul_rn(acc[4 * j + 2 * h + 1], g.alpha);
+      }
+    }
+    if (g.bias) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * (lane & 3);
+        acc[4 * j + 2 * h] = __fadd_rn(acc[4 * j + 2 * h], g.bias[min(n, g.N - 1)]);
+        acc[4 * j + 2 * h + 1] = __fadd_rn(acc[4 * j + 2 * h + 1], g.bias[min(n + 1, g.N - 1)]);
+      }
+    }
+    if (g.rowgroup) {
+      const float* rg = g.rowgroup + (long long)(m / g.rows_per_group) * g.N;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * (lane & 3);
+        acc[4 * j + 2 * h] = __fadd_rn(acc[4 * j + 2 * h], rg[min(n, g.N - 1)]);
+        acc[4 * j + 2 * h + 1] = __fadd_rn(acc[4 * j + 2 * h + 1], rg[min(n + 1, g.N - 1)]);
+      }
+    }
+  }
 #pragma unroll
   for (int p = 0; p < kPasses; ++p) {
     if constexpr (RES_TMA) {
@@ -144,7 +177,6 @@ __device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUten
       const int r = w * 16 + (lane >> 2) + 8 * h;
       const int m = row0 + r;
       if (m >= g.M) continue;
-      const float* rg = g.rowgroup ? g.rowgroup + (long long)(m / g.rows_per_group) * g.N : nullptr;
       const bf16* res =
           !RES_TMA && g.residual ? g.residual + (long long)bz * g.res_bstride + (long long)m * g.ldr : nullptr;
       uint8_t* srow = stg + r * 64;
@@ -154,13 +186,11 @@ __device__ __forceinline__ void gemm_epilogue_tma(const GemmArgs& g, const CUten
         const int sub = 8 * j / kSubCols;
         if (sub / kSubsPerPass != p) continue;
         const int n = n0 + 8 * j + 2 * (lane & 3);
-        float f0 = acc[4 * j + 2 * h] * g.alpha, f1 = acc[4 * j + 2 * h + 1] * g.alpha;
+        float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
         const int byte = (8 * j % kSubCols + 2 * (lane & 3)) * kEsz;
         uint8_t* dst = srow + (sub % kSubsPerPass) * kSubBytes + ((((byte >> 4) ^ sw)) << 4) + (byte & 15);
         if (n < g.N) {
           const bool two = n + 1 < g.N;
-          if (g.bias) { f0 += g.bias[n]; if (two) f1 += g.bias[n + 1]; }
-          if (rg) { f0 += rg[n]; if (two) f1 += rg[n + 1]; }
           if constexpr (RES_TMA) {
             const float2 rr = unpack_bf16(*reinterpret_cast<const uint32_t*>(dst));
             f0 += rr.x;

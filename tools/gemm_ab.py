@@ -1,6 +1,7 @@
 """Per-call inventory and A/B timing of the GEMM / implicit-convolution engine over one pre-training step.
 
     python tools/gemm_ab.py [--lib PATH ...] [--batch 16] [--iters 15] [--without-residual] [--out FILE]
+    python tools/gemm_ab.py --tile-cost [--tile-m 16384] [--lib PATH] [--iters 7] [--out FILE]
 
 Runs one eager pre-training step (bench.py's models and inputs, after one warm-up step) with ops.gemm, ops.conv3x3,
 ops.conv3x3_s2 and ops.conv3x3_wgrad wrapped, and records every call: shapes, operand majors, output dtype and mode,
@@ -14,6 +15,13 @@ SM clock are read in the same run.  Needs a GPU; fails without one.
 
 --without-residual replays every call that adds a residual a second time with residual=None, alternating with the
 original call on the same inputs, and reports per call and call-weighted per step what adding the residual costs.
+
+--tile-cost [--tile-m 16384] skips the step and times the engine alone (L2 flushed, median of --iters launches) at
+M = --tile-m for N in 320 ... 5120, every tile width BN the tile-width choice can take (forced with force_bn), K from 64
+to 2880, and bf16, bf16 + residual and fp32 outputs.  Per BN and output mode it fits time = rounds * (a + b * kchunks)
+by least squares (rounds = persistent-grid rounds, ceil(tiles / SMs); kchunks = K / 64) and reports a, the fixed cost
+per tile, and b, the cost per 64-deep k-chunk, in microseconds, with the worst relative residual of the fit.  Every
+sample goes into the --out report.
 """
 import argparse
 import ctypes
@@ -175,8 +183,66 @@ def stats(ts):
     return {"median_ms": round(ts[len(ts) // 2], 4), "min_ms": round(ts[0], 4), "max_ms": round(ts[-1], 4)}
 
 
+TILE_N = (320, 640, 960, 1280, 2560, 5120)
+TILE_K = (64, 128, 320, 640, 1280, 2880)
+TILE_MODES = ("bf16", "bf16_residual", "fp32")
+
+
+def tile_cost(args, handle):
+    """Fixed and per-chunk cost of an engine tile, fitted from a K sweep at fixed M x N (see the module docstring)."""
+    import numpy as np
+    from e4t_b200 import _lib, ops
+    _lib._lib = handle
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    M = args.tile_m
+    g = torch.Generator(device="cuda").manual_seed(7)
+    A = torch.randn(M, max(TILE_K), device="cuda", generator=g).mul_(0.2).bfloat16()
+    Bw = torch.randn(max(TILE_N), max(TILE_K), device="cuda", generator=g).mul_(0.2).bfloat16()
+    R = torch.randn(M, max(TILE_N), device="cuda", generator=g).mul_(0.2).bfloat16()
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")
+    samples = {}
+    for N in TILE_N:
+        for bn in range(64, 257, 32):
+            if bn > 2 * N:
+                continue
+            rounds = -(-(-(-M // 128) * -(-N // bn)) // sms)
+            for K in TILE_K:
+                a, b = A[:, :K].contiguous(), Bw[:N, :K].contiguous()
+                for mode in TILE_MODES:
+                    kw = dict(force_bn=bn, out_dtype=torch.float32 if mode == "fp32" else torch.bfloat16,
+                              residual=R[:, :N] if mode == "bf16_residual" else None)
+                    ts = []
+                    for it in range(args.iters + 1):             # the first launch warms up
+                        flush.zero_()
+                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                        e0.record()
+                        ops.gemm(a, b, **kw)
+                        e1.record()
+                        e1.synchronize()
+                        if it:
+                            ts.append(e0.elapsed_time(e1))
+                    ts.sort()
+                    samples.setdefault((bn, mode), []).append(
+                        dict(N=N, K=K, rounds=rounds, kchunks=K // 64, ms=ts[len(ts) // 2]))
+    fits = []
+    for (bn, mode), rows in sorted(samples.items()):
+        X = np.array([[r["rounds"], r["rounds"] * r["kchunks"]] for r in rows], dtype=np.float64)
+        y = np.array([r["ms"] * 1e3 for r in rows])
+        (ca, cb), *_ = np.linalg.lstsq(X, y, rcond=None)
+        worst = float(np.max(np.abs(X @ np.array([ca, cb]) - y) / y))
+        fits.append(dict(BN=bn, mode=mode, a_us=round(float(ca), 3), b_us=round(float(cb), 4), points=len(rows),
+                         worst_rel_resid=round(worst, 3)))
+    print(f"{'BN':>4s} {'mode':14s} {'a us':>8s} {'b us':>8s} {'pts':>4s} {'worst':>6s}")
+    for f in fits:
+        print(f"{f['BN']:4d} {f['mode']:14s} {f['a_us']:8.3f} {f['b_us']:8.4f} {f['points']:4d} "
+              f"{f['worst_rel_resid']:6.3f}")
+    return {"tile_m": M, "sms": sms, "fits": fits, "samples": {f"{k[0]}/{k[1]}": v for k, v in samples.items()}}
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--tile-cost", action="store_true", help="fit the per-tile and per-chunk cost instead of the step")
+    ap.add_argument("--tile-m", type=int, default=16384)
     ap.add_argument("--lib", action="append", default=[], help="libe4t_b200.so to time (repeat to A/B; first runs the step)")
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--iters", type=int, default=15)
@@ -192,6 +258,15 @@ def main():
     handles = [open_lib(p) for p in libs]
     _lib._lib = handles[0]
     report = {"card_before": card(), "batch": args.batch, "iters": args.iters, "libs": libs}
+    if args.tile_cost:
+        report["tile_cost"] = tile_cost(args, handles[0])
+        report["card_after"] = card()
+        print(json.dumps({"card_before": report["card_before"], "card_after": report["card_after"]}))
+        if args.out:
+            os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+            with open(args.out, "w") as f:
+                json.dump(report, f, indent=1)
+        return
     calls = inventory(args.batch)
     report["distinct_calls"] = len(calls)
     report["calls_per_step"] = sum(calls.values())
