@@ -534,11 +534,14 @@ static int launch_gemm(const CUtensorMap& mA, const CUtensorMap& mB, GemmArgs& g
                        bool im2col = false) {
   const int esz = g.out_mode == 0 ? 2 : 4;
   g.pair_store = (g.ldo % 2) == 0 && (g.batch == 1 || (g.out_bstride % 2) == 0) && ((uintptr_t)g.out % (2 * esz)) == 0;
-  // TMA addresses the output when its base is 16-byte aligned and its row pitch and batch stride are multiples of
-  // 16 bytes; anything else, or E4T_GEMM_EPI_PLAIN=0, takes the register epilogue.
+  // TMA addresses the output when its base is 16-byte aligned and its row width, row pitch and batch stride are
+  // multiples of 16 bytes; anything else, or E4T_GEMM_EPI_PLAIN=0, takes the register epilogue.  (The row width: on
+  // the H100 a TMA store whose row ends off a 16-byte boundary writes on to that boundary, so with a row pitch beyond
+  // N it overwrote up to 7 bf16 / 3 fp32 elements past N, the neighbouring columns of a column-slice output.)
   const char* p = getenv("E4T_GEMM_EPI_PLAIN");
   const bool want_tma = !(p && *p) || atoi(p) != 0;
-  g.epi_tma = want_tma && ((uintptr_t)g.out % 16) == 0 && (g.ldo * esz) % 16 == 0 && g.ldo >= g.N &&
+  g.epi_tma = want_tma && ((uintptr_t)g.out % 16) == 0 && (g.N * esz) % 16 == 0 && (g.ldo * esz) % 16 == 0 &&
+              g.ldo >= g.N &&
               (g.batch == 1 || (g.out_bstride > 0 && (g.out_bstride * esz) % 16 == 0));
   CUtensorMap mO;
   memset(&mO, 0, sizeof(mO));
@@ -598,7 +601,10 @@ extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int
   g.a_batched = (a_bstride != 0); g.b_batched = (b_bstride != 0);
   g.m_tiles = cdiv(M, kBM);
   g.kchunks = cdiv(K, kBK);
-  if (splits == 0 && out_mode == 2 && force_bn <= 0) splits = auto_splits(N, (long)g.m_tiles * batch, b_mn != 0, g.kchunks);
+  // every split's epilogue applies bias, row-group addend and residual: split-K takes none of them
+  const bool addends = bias || rowgroup || residual;
+  if (splits == 0 && out_mode == 2 && force_bn <= 0 && !addends)
+    splits = auto_splits(N, (long)g.m_tiles * batch, b_mn != 0, g.kchunks);
   if (splits < 1) splits = 1;
   if (splits > g.kchunks) splits = g.kchunks;
   g.kper = cdiv(g.kchunks, splits);
@@ -607,6 +613,7 @@ extern "C" int e4t_gemm_bf16(const void* A, const void* B, void* out, int M, int
   E4T_CHECK(g.BN >= 64 && g.BN <= 256 && (g.BN % (b_mn ? 64 : 32)) == 0, "e4t_gemm_bf16: bad BN %d", g.BN);
   g.n_tiles = cdiv(N, g.BN);
   E4T_CHECK(g.splits == 1 || out_mode == 2, "e4t_gemm_bf16: split-K requires atomic fp32 output");
+  E4T_CHECK(g.splits == 1 || !addends, "e4t_gemm_bf16: split-K would add bias / rowgroup / residual once per split");
   g.out = out; g.out_mode = out_mode; g.ldo = ldo; g.out_bstride = out_bstride;
   g.bias = bias; g.rowgroup = rowgroup; g.rows_per_group = rows_per_group > 0 ? rows_per_group : 1;
   g.residual = (const bf16*)residual; g.ldr = ldr; g.res_bstride = res_bstride;

@@ -134,8 +134,8 @@ class AttentionBlock(nn.Module):
         o = torch.empty((B, N, C), device=x.device, dtype=torch.bfloat16)
         # N % 8 != 0 (a latent with an odd side): the score and probability rows get a pitch of Np = N rounded up to 8
         # elements, which TMA and the softmax's vector loads need.  The pad columns of the scores are set to -inf after
-        # the GEMM (whose TMA epilogue may write zeros up to the next 16-byte boundary past N), so their probabilities
-        # are exact zeros; P·V reads K = N columns of P (its K tail is TMA out-of-bounds zero fill)
+        # the GEMM, so their probabilities are exact zeros; P·V reads K = N columns of P (its K tail is TMA
+        # out-of-bounds zero fill)
         Np = (N + 7) // 8 * 8
         chunk = max(1, ATTN_SCORE_BYTES // (N * Np * 4))
         for i in range(0, B, chunk):

@@ -24,15 +24,18 @@ def gemm(A, B, *, a_mn=False, b_mn=False, out=None, out_dtype=BF16, bias=None, r
 
     K-major operands are (.., rows, K) with K contiguous; MN-major operands are (.., K, rows) with rows
     contiguous (i.e. the transposed storage).  A 2-D operand is shared across the batch.
-    accumulate=True -> fp32 atomic accumulation into `out` (required for split-K).
+    accumulate=True -> fp32 atomic accumulation into `out` (required for split-K, which takes no bias, rowgroup or
+    residual).  out, residual, bias and rowgroup must cover (batch, M, N), N and ceil(M / rows_per_group) x N.
     """
     assert A.dtype == BF16 and B.dtype == BF16
     assert A.stride(-1) == 1 and B.stride(-1) == 1
+    if A.dim() == 3 and B.dim() == 3 and A.shape[0] != B.shape[0]:
+        raise ValueError(f"gemm: operands disagree on batch: A {tuple(A.shape)}, B {tuple(B.shape)}")
     batch = 1
     if A.dim() == 3:
         batch = A.shape[0]
     if B.dim() == 3:
-        batch = max(batch, B.shape[0])
+        batch = B.shape[0]
     if a_mn:
         K, M = A.shape[-2], A.shape[-1]
     else:
@@ -42,6 +45,16 @@ def gemm(A, B, *, a_mn=False, b_mn=False, out=None, out_dtype=BF16, bias=None, r
     else:
         N, Kb = B.shape[-2], B.shape[-1]
     assert K == Kb, (A.shape, B.shape, a_mn, b_mn)
+    # The library takes only pointers and strides: a tensor smaller than the call would be read or written past its end
+    if out is not None and tuple(out.shape) != ((batch, M, N) if out.dim() == 3 else (M, N) if batch == 1 else None):
+        raise ValueError(f"gemm: out {tuple(out.shape)} is not (batch, M, N) = ({batch}, {M}, {N})")
+    if residual is not None and (tuple(residual.shape[-2:]) != (M, N) or residual.dim() not in (2, 3)
+                                 or (residual.dim() == 3 and residual.shape[0] != batch)):
+        raise ValueError(f"gemm: residual {tuple(residual.shape)} does not cover ({batch}, {M}, {N})")
+    if bias is not None and bias.numel() != N:
+        raise ValueError(f"gemm: bias has {bias.numel()} elements, N = {N}")
+    if rowgroup is not None and (rows_per_group < 1 or rowgroup.numel() != -(-M // rows_per_group) * N):
+        raise ValueError(f"gemm: rowgroup {tuple(rowgroup.shape)} is not ceil({M} / {rows_per_group}) rows of {N}")
     a_bs = A.stride(0) if A.dim() == 3 and batch > 1 else 0
     b_bs = B.stride(0) if B.dim() == 3 and batch > 1 else 0
     if accumulate:
