@@ -624,10 +624,13 @@ extern "C" int e4t_conv_out_bwd(const float* dy, const float* w, void* dx, int B
 // ---------------------------------------------------------------------------------------------
 __global__ void adamw_tick_kernel(int* step) { *step += 1; }
 __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                             float* __restrict__ v, long n, float lr, float beta1, float beta2, float eps, float wd,
-                             const int* __restrict__ step_ptr, int step_host, float grad_scale) {
-  // bias corrections from the DEVICE step counter when given (CUDA-graph replays advance it), else the host value
+                             float* __restrict__ v, long n, float lr_host, float beta1, float beta2, float eps, float wd,
+                             const int* __restrict__ step_ptr, int step_host, float grad_scale,
+                             const float* __restrict__ lr_ptr) {
+  // bias corrections from the DEVICE step counter when given (CUDA-graph replays advance it), else the host value;
+  // likewise the learning rate (written by adamw_sched_tick_kernel when a schedule is followed)
   const int step = step_ptr ? *step_ptr : step_host;
+  const float lr = lr_ptr ? *lr_ptr : lr_host;
   const float bc1 = 1.f - powf(beta1, (float)step);
   const float bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
   const long n4 = n / 4;
@@ -668,7 +671,8 @@ extern "C" int e4t_adamw_step(float* p, const float* g, float* m, float* v, long
   E4T_CHECK(((uintptr_t)p % 16) == 0 && ((uintptr_t)g % 16) == 0 && ((uintptr_t)m % 16) == 0 && ((uintptr_t)v % 16) == 0,
             "e4t_adamw_step: buffers must be 16-byte aligned");
   adamw_kernel<<<grid_for(n / 4 + 1, 256), 256, 0, (cudaStream_t)stream_>>>(p, g, m, v, n, lr, beta1, beta2, eps,
-                                                                            weight_decay, nullptr, step, grad_scale);
+                                                                            weight_decay, nullptr, step, grad_scale,
+                                                                            nullptr);
   E4T_COUNT_LAUNCH();
   E4T_LAUNCH_CHECK();
   return 0;
@@ -682,7 +686,200 @@ extern "C" int e4t_adamw_step_dev(float* p, const float* g, float* m, float* v, 
   adamw_tick_kernel<<<1, 1, 0, (cudaStream_t)stream_>>>(step_dev);
   E4T_COUNT_LAUNCH();
   adamw_kernel<<<grid_for(n / 4 + 1, 256), 256, 0, (cudaStream_t)stream_>>>(p, g, m, v, n, lr, beta1, beta2, eps,
-                                                                            weight_decay, step_dev, 0, grad_scale);
+                                                                            weight_decay, step_dev, 0, grad_scale,
+                                                                            nullptr);
+  E4T_COUNT_LAUNCH();
+  E4T_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- learning-rate schedules (diffusers 0.14 get_scheduler == transformers.optimization; e4t_b200/optim.py) --------
+// kind: 0 constant, 1 constant_with_warmup, 2 linear, 3 cosine, 4 cosine_with_restarts, 5 polynomial.
+struct LrSchedule {
+  int kind, warmup, total;
+  double cycles, power, lr_end;
+};
+// λ(t) after t optimiser steps, in fp64, the same operations as e4t_b200.optim.lr_lambda
+__device__ double lr_lambda(const LrSchedule& s, int t, double lr) {
+  if (s.kind == 0) return 1.0;
+  if (t < s.warmup) return (double)t / (double)max(1, s.warmup);
+  if (s.kind == 1) return 1.0;
+  if (s.kind == 2) return fmax(0.0, (double)(s.total - t) / (double)max(1, s.total - s.warmup));
+  if (s.kind == 5) {
+    if (t > s.total) return s.lr_end / lr;
+    const double pct_remaining = 1.0 - (double)(t - s.warmup) / (double)(s.total - s.warmup);
+    return ((lr - s.lr_end) * pow(pct_remaining, s.power) + s.lr_end) / lr;
+  }
+  const double progress = (double)(t - s.warmup) / (double)max(1, s.total - s.warmup);
+  if (s.kind == 3) return fmax(0.0, 0.5 * (1.0 + cos(M_PI * s.cycles * 2.0 * progress)));
+  if (progress >= 1.0) return 0.0;
+  return fmax(0.0, 0.5 * (1.0 + cos(M_PI * fmod(s.cycles * progress, 1.0))));
+}
+// *step_dev holds the steps already taken: the step about to run uses lr * λ(*step_dev) (torch LambdaLR stepped after
+// optimizer.step()), written to *lr_dev for the update kernel and for the caller; then the counter advances.
+__global__ void adamw_sched_tick_kernel(int* step, float* lr_out, float lr, LrSchedule s) {
+  const int t = *step;
+  *lr_out = (float)((double)lr * lr_lambda(s, t, (double)lr));
+  *step = t + 1;
+}
+static int check_schedule(const char* fn, const LrSchedule& s, float lr) {
+  E4T_CHECK(s.kind >= 0 && s.kind <= 5, "%s: unknown schedule kind %d (0 constant, 1 constant_with_warmup, 2 linear, "
+            "3 cosine, 4 cosine_with_restarts, 5 polynomial)", fn, s.kind);
+  E4T_CHECK(s.warmup >= 0, "%s: warm-up of %d steps", fn, s.warmup);
+  E4T_CHECK(s.kind < 2 || s.total >= 1, "%s: schedule kind %d needs a positive total step count, got %d", fn, s.kind,
+            s.total);
+  E4T_CHECK(s.kind != 5 || ((double)lr > s.lr_end && s.total != s.warmup),
+            "%s: polynomial decay needs lr > lr_end and total != warm-up steps", fn);
+  return 0;
+}
+
+extern "C" int e4t_adamw_step_sched(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1,
+                                    float beta2, float eps, float weight_decay, int* step_dev, float* lr_dev,
+                                    int sched_kind, int warmup, int total, double num_cycles, double power,
+                                    double lr_end, float grad_scale, void* stream_) {
+  E4T_CHECK(((uintptr_t)p % 16) == 0 && ((uintptr_t)g % 16) == 0 && ((uintptr_t)m % 16) == 0 && ((uintptr_t)v % 16) == 0,
+            "e4t_adamw_step_sched: buffers must be 16-byte aligned");
+  const LrSchedule s{sched_kind, warmup, total, num_cycles, power, lr_end};
+  if (const int r = check_schedule("e4t_adamw_step_sched", s, lr)) return r;
+  adamw_sched_tick_kernel<<<1, 1, 0, (cudaStream_t)stream_>>>(step_dev, lr_dev, lr, s);
+  E4T_COUNT_LAUNCH();
+  adamw_kernel<<<grid_for(n / 4 + 1, 256), 256, 0, (cudaStream_t)stream_>>>(p, g, m, v, n, lr, beta1, beta2, eps,
+                                                                            weight_decay, step_dev, 0, grad_scale,
+                                                                            lr_dev);
+  E4T_COUNT_LAUNCH();
+  E4T_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// 8-bit AdamW: block-wise dynamic quantisation of m and v (Dettmers et al. 2022; DESIGN.md, "Optimiser options")
+// m, v are uint8 codes into two sorted 256-entry fp32 maps (signed for m, unsigned for v, e4t_b200.optim.dynamic_map)
+// times one fp32 absmax per 256-element block.  One warp owns one block: lane l holds elements 4l..4l+3 and
+// 128+4l..128+4l+3 (float4 / uint32 loads, fully coalesced), the block absmax is a warp-shuffle max.
+// Traffic: p r/w 8 B + g 4 B + two codes r/w 4 B = 16 B per element (fp32 AdamW: 28 B).
+// ---------------------------------------------------------------------------------------------
+constexpr int Q8_BLOCK = 256;
+// The maps' structure: decade i = 0..6 holds K_i values 10^(i-6) * (0.1 + 0.9 (j + 0.5) / K_i), j < K_i, with
+// K_i = 2^i (signed) or 2^(i+1) (unsigned).  Per map and decade: {scale, bias, first magnitude index, K_i - 1} such that
+// j ~ rint(|x| * scale - bias).
+__device__ __forceinline__ float4 q8_decade(int is_unsigned, int i) {
+  const float K = (float)((1 + is_unsigned) << i);
+  const float start = is_unsigned ? (float)((2 << i) - 2) : (float)((1 << i) - 1);
+  return make_float4((float)(exp10((double)(6 - i)) * K / 0.9), (float)(0.1 * K / 0.9 + 0.5), start, K - 1.f);
+}
+// Nearest map entry to x (ties to the lower index).  The code is computed arithmetically from the map's structure and
+// is off by at most one entry (rounding near decade and step boundaries), so one comparison with the neighbour on x's
+// side of it settles it: two shared-memory reads instead of an 8-step binary search.
+__device__ __forceinline__ uint32_t q8_code(float x, const float* __restrict__ map, const float4* __restrict__ dec,
+                                            bool is_signed) {
+  const float a = fabsf(x);
+  const int i = (a >= 1e-6f) + (a >= 1e-5f) + (a >= 1e-4f) + (a >= 1e-3f) + (a >= 1e-2f) + (a >= 1e-1f);
+  const float4 d = dec[i];
+  const int q = (int)(d.z + fminf(fmaxf(rintf(fmaf(a, d.x, -d.y)), 0.f), d.w));
+  // signed: [-1, -mag[126..1], 0, mag[0..126], 1]; unsigned: [0, mag[0..253], 1]
+  int c = is_signed ? (x < 0.f ? 127 - q : 128 + q) : 1 + q;
+  const float mc = map[c];
+  if (x > mc) {
+    if (map[c + 1] - x < x - mc) ++c;
+  } else if (x < mc) {
+    if (x - map[c - 1] <= mc - x) --c;
+  }
+  return (uint32_t)c;
+}
+
+__global__ void __launch_bounds__(256) adamw8bit_kernel(float* __restrict__ p, const float* __restrict__ g,
+                                                        uint8_t* __restrict__ mq, uint8_t* __restrict__ vq,
+                                                        float* __restrict__ m_absmax, float* __restrict__ v_absmax,
+                                                        const float* __restrict__ qmap_m,
+                                                        const float* __restrict__ qmap_v, long nblocks, float beta1,
+                                                        float beta2, float eps, float wd,
+                                                        const int* __restrict__ step_ptr,
+                                                        const float* __restrict__ lr_ptr, float grad_scale) {
+  __shared__ float smap[2][256];
+  __shared__ float4 sdec[2][8];
+  for (int i = threadIdx.x; i < 512; i += blockDim.x) smap[i >> 8][i & 255] = (i < 256 ? qmap_m : qmap_v)[i & 255];
+  if (threadIdx.x < 14) sdec[threadIdx.x / 7][threadIdx.x % 7] = q8_decade(threadIdx.x / 7, threadIdx.x % 7);
+  __syncthreads();
+  const int step = *step_ptr;
+  const float lr = *lr_ptr;
+  const float bc1 = 1.f - powf(beta1, (float)step);
+  const float bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
+  const float decay = 1.f - lr * wd, step_size = lr / bc1;
+  const int lane = threadIdx.x & 31;
+  const long nwarps = ((long)gridDim.x * blockDim.x) >> 5;
+  for (long b = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < nblocks; b += nwarps) {
+    const float am_old = m_absmax[b], av_old = v_absmax[b];
+    float pa[8], ma[8], va[8];
+    float am = 0.f, av = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long e = b * Q8_BLOCK + h * 128 + lane * 4;
+      const float4 pp = *reinterpret_cast<const float4*>(p + e);
+      const float4 gg = *reinterpret_cast<const float4*>(g + e);
+      const uint32_t mc = *reinterpret_cast<const uint32_t*>(mq + e), vc = *reinterpret_cast<const uint32_t*>(vq + e);
+      const float pin[4] = {pp.x, pp.y, pp.z, pp.w}, gin[4] = {gg.x, gg.y, gg.z, gg.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int k = h * 4 + j;
+        // adamw_kernel's update on the dequantised moments
+        const float gr = gin[j] * grad_scale;
+        float pv = pin[j] * decay;
+        const float mv = beta1 * (smap[0][(mc >> (8 * j)) & 255] * am_old) + (1.f - beta1) * gr;
+        const float vv = beta2 * (smap[1][(vc >> (8 * j)) & 255] * av_old) + (1.f - beta2) * gr * gr;
+        pv -= step_size * mv / (sqrtf(vv) / bc2_sqrt + eps);
+        pa[k] = pv;
+        ma[k] = mv;
+        va[k] = vv;
+        am = fmaxf(am, fabsf(mv));
+        av = fmaxf(av, vv);
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
+      av = fmaxf(av, __shfl_xor_sync(0xffffffffu, av, o));
+    }
+    const float im = am > 0.f ? 1.f / am : 0.f, iv = av > 0.f ? 1.f / av : 0.f;  // an all-zero block codes 0
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long e = b * Q8_BLOCK + h * 128 + lane * 4;
+      uint32_t mc = 0, vc = 0;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        mc |= q8_code(ma[h * 4 + j] * im, smap[0], sdec[0], true) << (8 * j);
+        vc |= q8_code(va[h * 4 + j] * iv, smap[1], sdec[1], false) << (8 * j);
+      }
+      *reinterpret_cast<float4*>(p + e) = make_float4(pa[h * 4], pa[h * 4 + 1], pa[h * 4 + 2], pa[h * 4 + 3]);
+      *reinterpret_cast<uint32_t*>(mq + e) = mc;
+      *reinterpret_cast<uint32_t*>(vq + e) = vc;
+    }
+    if (lane == 0) {
+      m_absmax[b] = am;
+      v_absmax[b] = av;
+    }
+  }
+}
+
+extern "C" int e4t_adamw8bit_step_sched(float* p, const float* g, unsigned char* m_codes, unsigned char* v_codes,
+                                        float* m_absmax, float* v_absmax, const float* qmap_m, const float* qmap_v,
+                                        long long n, float lr, float beta1, float beta2, float eps,
+                                        float weight_decay, int* step_dev, float* lr_dev, int sched_kind, int warmup,
+                                        int total, double num_cycles, double power, double lr_end, float grad_scale,
+                                        void* stream_) {
+  E4T_CHECK(n % Q8_BLOCK == 0, "e4t_adamw8bit_step_sched: n = %lld is not a multiple of %d (one absmax per block of "
+            "%d elements)", n, Q8_BLOCK, Q8_BLOCK);
+  E4T_CHECK(((uintptr_t)p % 16) == 0 && ((uintptr_t)g % 16) == 0 && ((uintptr_t)m_codes % 16) == 0 &&
+                ((uintptr_t)v_codes % 16) == 0 && ((uintptr_t)m_absmax % 16) == 0 && ((uintptr_t)v_absmax % 16) == 0 &&
+                ((uintptr_t)qmap_m % 16) == 0 && ((uintptr_t)qmap_v % 16) == 0,
+            "e4t_adamw8bit_step_sched: buffers must be 16-byte aligned");
+  const LrSchedule s{sched_kind, warmup, total, num_cycles, power, lr_end};
+  if (const int r = check_schedule("e4t_adamw8bit_step_sched", s, lr)) return r;
+  adamw_sched_tick_kernel<<<1, 1, 0, (cudaStream_t)stream_>>>(step_dev, lr_dev, lr, s);
+  E4T_COUNT_LAUNCH();
+  const long nblocks = n / Q8_BLOCK;
+  adamw8bit_kernel<<<grid_for(nblocks * 32, 256), 256, 0, (cudaStream_t)stream_>>>(
+      p, g, m_codes, v_codes, m_absmax, v_absmax, qmap_m, qmap_v, nblocks, beta1, beta2, eps, weight_decay, step_dev,
+      lr_dev, grad_scale);
   E4T_COUNT_LAUNCH();
   E4T_LAUNCH_CHECK();
   return 0;

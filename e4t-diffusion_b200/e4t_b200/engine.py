@@ -15,6 +15,7 @@ import torch.nn.functional as F
 
 from . import functional as FN
 from . import ops
+from . import optim
 from ._lib import E4TError
 
 PLACEHOLDER_FALLBACK = 49408
@@ -50,7 +51,14 @@ def shard_seed(base_seed, rank):
 class FlatAdamW:
     """torch.optim.AdamW semantics over a flat arena (amsgrad=False).  `params`: iterable of nn.Parameter."""
 
-    def __init__(self, params, lr=1.6e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, process_group=None):
+    def __init__(self, params, lr=1.6e-5, betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, process_group=None,
+                 lr_scheduler="constant", lr_warmup_steps=0, max_train_steps=None, optim_bits=32):
+        """lr_scheduler / lr_warmup_steps / max_train_steps: --lr_scheduler, --lr_warmup_steps, --max_train_steps
+        (e4t_b200.optim.SCHEDULES), evaluated on the device from `step_dev`.  optim_bits=8: --use_8bit_adam, block-wise
+        8-bit moments (DESIGN.md, "Optimiser options")."""
+        self._sched_kind = optim.check_schedule(lr_scheduler, lr_warmup_steps, max_train_steps, lr)
+        if optim_bits not in (8, 32):
+            raise ValueError(f"optim_bits must be 32 or 8, got {optim_bits}")
         seen, plist = set(), []
         for p in params:
             if p.requires_grad and id(p) not in seen:
@@ -62,6 +70,8 @@ class FlatAdamW:
         self.params = plist
         self.lr, self.betas, self.weight_decay, self.eps = lr, betas, weight_decay, eps
         self.process_group = process_group
+        self.lr_scheduler, self.lr_warmup_steps = lr_scheduler, int(lr_warmup_steps)
+        self.max_train_steps, self.optim_bits = max_train_steps, optim_bits
         # storages shared by several parameters (E4TEncoder's stacked first_linears) must stay contiguous: group by
         # untyped storage and move each storage once
         groups = {}
@@ -69,18 +79,30 @@ class FlatAdamW:
             groups.setdefault(p.untyped_storage().data_ptr(), []).append(p)
         total = 0
         layout = []
+        # 8-bit moments keep one absmax per 256 elements: padding each storage to 256 keeps storages out of each
+        # other's blocks
+        pad = optim.BLOCK if optim_bits == 8 else 4
         for sp, ps in groups.items():
             base = min(p.data_ptr() for p in ps)
             end = max(p.data_ptr() + p.numel() * 4 for p in ps)
             n = (end - base) // 4
-            n_pad = (n + 3) // 4 * 4
+            n_pad = (n + pad - 1) // pad * pad
             layout.append((ps, base, n, total))
             total += n_pad
         self.numel = total
         self.arena = torch.zeros(total, device=dev, dtype=torch.float32)
         self.grad = torch.zeros(total, device=dev, dtype=torch.float32)
-        self.exp_avg = torch.zeros(total, device=dev, dtype=torch.float32)
-        self.exp_avg_sq = torch.zeros(total, device=dev, dtype=torch.float32)
+        if optim_bits == 8:
+            self.exp_avg = self.exp_avg_sq = None
+            self.m_codes = torch.zeros(total, device=dev, dtype=torch.uint8)   # zero codes and absmax decode to 0
+            self.v_codes = torch.zeros(total, device=dev, dtype=torch.uint8)
+            self.m_absmax = torch.zeros(total // optim.BLOCK, device=dev, dtype=torch.float32)
+            self.v_absmax = torch.zeros(total // optim.BLOCK, device=dev, dtype=torch.float32)
+            self.qmap_m = optim.dynamic_map(signed=True).to(dev)
+            self.qmap_v = optim.dynamic_map(signed=False).to(dev)
+        else:
+            self.exp_avg = torch.zeros(total, device=dev, dtype=torch.float32)
+            self.exp_avg_sq = torch.zeros(total, device=dev, dtype=torch.float32)
         with torch.no_grad():
             for ps, base, n, off in layout:
                 for p in ps:
@@ -97,7 +119,10 @@ class FlatAdamW:
             for p in ps:
                 self.offsets[id(p)] = (off + (p.data_ptr() - self.arena.data_ptr()) // 4 - off, p.numel())
         self.step_count = 0
-        self.step_dev = torch.zeros(1, device=dev, dtype=torch.int32)   # device-side counter: graph-replayable
+        # device-side counter: graph-replayable.  It counts every optimiser step run, enable_cuda_graph's warm-up
+        # steps included, and is the position in the lr schedule
+        self.step_dev = torch.zeros(1, device=dev, dtype=torch.int32)
+        self.lr_dev = torch.full((1,), float(lr), device=dev, dtype=torch.float32)  # lr of the last scheduled step
         FN.DIRECT_GRAD_WRITE = True     # .grad views are zeroed by zero_grad(); WO kernels write them directly
         FN.bump_param_epoch()
         # modules that cache views of re-homed storages refresh themselves lazily (E4TEncoder._stacked)
@@ -121,29 +146,64 @@ class FlatAdamW:
         mine = sum(self.offsets[i][1] for i in ids)
         return (end + 3) // 4 * 4 if inside == mine else None
 
+    def _sched(self):
+        return (self._sched_kind, self.lr_warmup_steps, self.max_train_steps or 0,
+                optim.NUM_CYCLES.get(self.lr_scheduler, 0.0), optim.POWER, optim.LR_END)
+
     def step(self, grad_scale=1.0):
         self.step_count += 1
-        ops.adamw_step_dev(self.arena, self.grad, self.exp_avg, self.exp_avg_sq, self.lr, self.betas[0], self.betas[1],
-                           self.eps, self.weight_decay, self.step_dev, grad_scale)
+        if self.optim_bits == 8:
+            ops.adamw8bit_step_sched(self.arena, self.grad, self.m_codes, self.v_codes, self.m_absmax, self.v_absmax,
+                                     self.qmap_m, self.qmap_v, self.lr, self.betas[0], self.betas[1], self.eps,
+                                     self.weight_decay, self.step_dev, self.lr_dev, self._sched(), grad_scale)
+        elif self.lr_scheduler != "constant":
+            ops.adamw_step_sched(self.arena, self.grad, self.exp_avg, self.exp_avg_sq, self.lr, self.betas[0],
+                                 self.betas[1], self.eps, self.weight_decay, self.step_dev, self.lr_dev, self._sched(),
+                                 grad_scale)
+        else:
+            ops.adamw_step_dev(self.arena, self.grad, self.exp_avg, self.exp_avg_sq, self.lr, self.betas[0],
+                               self.betas[1], self.eps, self.weight_decay, self.step_dev, grad_scale)
         FN.bump_param_epoch()
+
+    def get_last_lr(self):
+        """[lr * λ(t)] after t steps: the lr the next step runs at (what the reference logs as train/lr)."""
+        t = int(self.step_dev.item())
+        return [self.lr * optim.lr_lambda(self.lr_scheduler, t, self.lr_warmup_steps, self.max_train_steps, self.lr)]
 
 
     # ---- checkpoint / resume (pretrain_e4t.py:536-558 resumes optimizer state through accelerator.load_state) ------
+    _STATE_8BIT = ("m_codes", "v_codes", "m_absmax", "v_absmax", "qmap_m", "qmap_v")
+
     def state_dict(self):
         """Moments and step count (clones, not arena views).  Parameters themselves travel in weight_offsets.pt /
-        encoder.pt; `numel` guards against loading into a differently laid-out arena."""
-        return dict(numel=self.numel, step=self.step_count, exp_avg=self.exp_avg.detach().clone(),
-                    exp_avg_sq=self.exp_avg_sq.detach().clone(), lr=self.lr, betas=self.betas,
-                    weight_decay=self.weight_decay, eps=self.eps)
+        encoder.pt; `numel` guards against loading into a differently laid-out arena.  `step` is the device counter:
+        CUDA-graph replays advance it and not the host's step_count."""
+        sd = dict(numel=self.numel, step=int(self.step_dev.item()), optim_bits=self.optim_bits, lr=self.lr,
+                  betas=self.betas, weight_decay=self.weight_decay, eps=self.eps, lr_scheduler=self.lr_scheduler,
+                  lr_warmup_steps=self.lr_warmup_steps, max_train_steps=self.max_train_steps)
+        names = self._STATE_8BIT if self.optim_bits == 8 else ("exp_avg", "exp_avg_sq")
+        sd.update({k: getattr(self, k).detach().clone() for k in names})
+        return sd
 
     def load_state_dict(self, sd):
+        bits = int(sd.get("optim_bits", 32))
+        if bits != self.optim_bits:
+            raise ValueError(f"optimizer state has {bits}-bit moments, this optimizer keeps {self.optim_bits}-bit "
+                             "moments (use_8bit_adam must match the run that saved it)")
         if int(sd["numel"]) != self.numel:
             raise ValueError(f"optimizer arena size mismatch: checkpoint {sd['numel']} vs {self.numel}")
-        self.exp_avg.copy_(sd["exp_avg"])
-        self.exp_avg_sq.copy_(sd["exp_avg_sq"])
+        if bits == 8:
+            for k in ("qmap_m", "qmap_v"):
+                if not torch.equal(sd[k].to(getattr(self, k).device), getattr(self, k)):
+                    raise ValueError(f"optimizer state {k} is not the dynamic quantisation map this optimizer codes with")
+        for k in self._STATE_8BIT[:4] if bits == 8 else ("exp_avg", "exp_avg_sq"):
+            getattr(self, k).copy_(sd[k])
         self.step_count = int(sd["step"])
         self.step_dev.fill_(self.step_count)
-        for k in ("lr", "betas", "weight_decay", "eps"):
+        if "lr_scheduler" in sd:
+            self._sched_kind = optim.check_schedule(sd["lr_scheduler"], sd["lr_warmup_steps"], sd["max_train_steps"],
+                                                    sd.get("lr", self.lr))
+        for k in ("lr", "betas", "weight_decay", "eps", "lr_scheduler", "lr_warmup_steps", "max_train_steps"):
             if k in sd:
                 setattr(self, k, tuple(sd[k]) if k == "betas" else sd[k])
 
@@ -167,7 +227,11 @@ class PretrainStep:
     def __init__(self, unet, e4t_encoder, text_encoder, placeholder_token_id, class_token_id, lr=1.6e-5,
                  betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, domain_embed_scale=0.1, reg_lambda=0.01,
                  bos_id=49406, eos_id=49407, weight_dtype=torch.bfloat16, optimizer=True, tune_unet=False,
-                 max_grad_norm=None, vae=None, train_text_encoder=False):
+                 max_grad_norm=None, vae=None, train_text_encoder=False, use_8bit_adam=False, lr_scheduler="constant",
+                 lr_warmup_steps=0, max_train_steps=None):
+        # use_8bit_adam / lr_scheduler / lr_warmup_steps / max_train_steps: the optimiser flags of pretrain_e4t.py and
+        # tuning_e4t.py (FlatAdamW); refused before anything is built
+        optim.check_schedule(lr_scheduler, lr_warmup_steps, max_train_steps, lr)
         self.unet, self.enc, self.text = unet, e4t_encoder, text_encoder
         # vae: an e4t AutoencoderKL; with it, a batch without "latents" is encoded on the device (pretrain_e4t.py:598-599)
         self.vae = vae
@@ -195,7 +259,9 @@ class PretrainStep:
         params = trainable_parameters(unet, e4t_encoder, tune_unet)
         if self.train_text_encoder:
             params += list(self.text.parameters())                                       # tuning_e4t.py:144-146
-        self.opt = FlatAdamW(params, lr=lr, betas=betas, weight_decay=weight_decay, eps=eps) if optimizer else None
+        self.opt = FlatAdamW(params, lr=lr, betas=betas, weight_decay=weight_decay, eps=eps, lr_scheduler=lr_scheduler,
+                             lr_warmup_steps=lr_warmup_steps, max_train_steps=max_train_steps,
+                             optim_bits=8 if use_8bit_adam else 32) if optimizer else None
         self._graph = None
         self.wo_bank = None
         self._wo_factor_exchange = False

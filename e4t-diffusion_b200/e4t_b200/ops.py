@@ -10,6 +10,8 @@ import torch
 from . import _lib
 from ._lib import c_float, c_int, c_ll, c_void_p, ptr, stream
 
+c_double = ctypes.c_double
+
 BF16 = torch.bfloat16
 F32 = torch.float32
 
@@ -378,6 +380,33 @@ def adamw_step_dev(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step_dev, gr
     assert p.dtype == F32 and step_dev.dtype == torch.int32
     _lib.call("e4t_adamw_step_dev", ptr(p), ptr(g), ptr(m), ptr(v), c_ll(p.numel()), c_float(lr), c_float(beta1),
               c_float(beta2), c_float(eps), c_float(weight_decay), ptr(step_dev), c_float(grad_scale), stream())
+
+
+def _sched_args(sched):
+    kind, warmup, total, cycles, power, lr_end = sched
+    return c_int(kind), c_int(warmup), c_int(total), c_double(cycles), c_double(power), c_double(lr_end)
+
+
+def adamw_step_sched(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step_dev, lr_dev, sched, grad_scale=1.0):
+    """adamw_step_dev following a learning-rate schedule on the device: `sched` = (kind, warmup, total, num_cycles,
+    power, lr_end) (e4t_b200.optim); the lr each call uses is written to `lr_dev` (fp32, 1 element)."""
+    assert p.dtype == F32 and step_dev.dtype == torch.int32 and lr_dev.dtype == F32
+    _lib.call("e4t_adamw_step_sched", ptr(p), ptr(g), ptr(m), ptr(v), c_ll(p.numel()), c_float(lr), c_float(beta1),
+              c_float(beta2), c_float(eps), c_float(weight_decay), ptr(step_dev), ptr(lr_dev), *_sched_args(sched),
+              c_float(grad_scale), stream())
+
+
+def adamw8bit_step_sched(p, g, m_codes, v_codes, m_absmax, v_absmax, qmap_m, qmap_v, lr, beta1, beta2, eps,
+                         weight_decay, step_dev, lr_dev, sched, grad_scale=1.0):
+    """8-bit AdamW (block-wise quantised moments, one absmax per 256 elements) with a schedule as adamw_step_sched."""
+    assert p.dtype == F32 and g.dtype == F32 and m_codes.dtype == torch.uint8 and v_codes.dtype == torch.uint8
+    assert m_absmax.dtype == F32 and v_absmax.dtype == F32 and qmap_m.numel() == 256 and qmap_v.numel() == 256
+    n = p.numel()
+    if not (g.numel() == m_codes.numel() == v_codes.numel() == n and m_absmax.numel() == v_absmax.numel() == n // 256):
+        raise ValueError(f"adamw8bit_step_sched: {n} parameters need {n} gradients and codes and {n // 256} absmax")
+    _lib.call("e4t_adamw8bit_step_sched", ptr(p), ptr(g), ptr(m_codes), ptr(v_codes), ptr(m_absmax), ptr(v_absmax),
+              ptr(qmap_m), ptr(qmap_v), c_ll(n), c_float(lr), c_float(beta1), c_float(beta2), c_float(eps),
+              c_float(weight_decay), ptr(step_dev), ptr(lr_dev), *_sched_args(sched), c_float(grad_scale), stream())
 
 
 # ----------------------------------------------------------------------------------------------

@@ -212,6 +212,22 @@ int e4t_adamw_step(float* p, const float* g, float* m, float* v, long long n, fl
 /* Same with the step counter in device memory (*step_dev is incremented, then used): CUDA-graph replayable. */
 int e4t_adamw_step_dev(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
                        float eps, float weight_decay, int* step_dev, float grad_scale, void* stream);
+/* --lr_scheduler / --lr_warmup_steps (get_scheduler at pretrain_e4t.py:402-407): a tick kernel evaluates the factor
+ * λ(*step_dev) of schedule sched_kind (0 constant, 1 constant_with_warmup, 2 linear, 3 cosine, 4 cosine_with_restarts,
+ * 5 polynomial; warm-up `warmup`, `total` = max_train_steps, num_cycles, power, lr_end) in fp64, writes lr * λ to
+ * *lr_dev and increments *step_dev; the update then reads both from the device: CUDA-graph replays follow the
+ * schedule. */
+int e4t_adamw_step_sched(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
+                         float eps, float weight_decay, int* step_dev, float* lr_dev, int sched_kind, int warmup,
+                         int total, double num_cycles, double power, double lr_end, float grad_scale, void* stream);
+/* --use_8bit_adam (bnb.optim.AdamW8bit at pretrain_e4t.py:380-387): block-wise 8-bit moments.  m_codes / v_codes
+ * [n] index the sorted 256-entry maps qmap_m (signed) / qmap_v (unsigned); m_absmax / v_absmax [n / 256] scale each
+ * block of 256 elements.  n must be a multiple of 256 and every buffer 16-byte aligned.  Schedule as above. */
+int e4t_adamw8bit_step_sched(float* p, const float* g, unsigned char* m_codes, unsigned char* v_codes, float* m_absmax,
+                             float* v_absmax, const float* qmap_m, const float* qmap_v, long long n, float lr,
+                             float beta1, float beta2, float eps, float weight_decay, int* step_dev, float* lr_dev,
+                             int sched_kind, int warmup, int total, double num_cycles, double power, double lr_end,
+                             float grad_scale, void* stream);
 
 #ifdef __cplusplus
 }
