@@ -17,10 +17,11 @@
 // same kernel stages dSᵀ in shared memory and reduces dQ += dS·K into an fp32 buffer with atomics.  The two-kernel form
 // computes dQ in a kernel of its own (CTA = 64 queries, loop over key blocks).
 //
-// Which shapes run here: everything except the non-causal forward and single-pass backward with dh = 40 or 80 and N, M
-// multiples of 128 and >= 512 (the 4096-token level-0 and 1024-token level-1 self-attention; for dh = 80 only grids of
-// at least half as many 128-query CTAs as SMs), which the entry points below hand to the warpgroup kernels of
-// attention_wgmma.cu unless a switch (see "Runtime switches") keeps them here.
+// Which shapes run here: everything except the non-causal forward and single-pass backward with dh = 40, 64 or 80 and
+// N, M multiples of 128 and >= 512 (the 4096-token level-0 and 1024-token level-1 self-attention of SD 1.x, the SD 2.x
+// self-attention from 512 tokens up; for dh = 64 and 80 only grids of at least half as many 128-query CTAs as SMs),
+// which the entry points below hand to the warpgroup kernels of attention_wgmma.cu unless a switch (see "Runtime
+// switches") keeps them here.  With dh = 64 that leaves the 77-key cross-attention and the shorter SD 2.x levels to this file.
 #include "attention.cuh"
 #include <math.h>
 #include <stdlib.h>

@@ -22,8 +22,8 @@ struct AttnArgs {
 };
 
 // Warpgroup (wgmma + TMA) kernels for long non-causal self-attention, csrc/attention_wgmma.cu.
-// attn_wgmma_shape_ok: the shapes those kernels take (dh = 40 or 80, N and M multiples of 128 and >= 512; for dh = 80
-// also a grid of (N / 128) x H x B CTAs of at least half the SM count).
+// attn_wgmma_shape_ok: the shapes those kernels take (dh = 40, 64 or 80, N and M multiples of 128 and >= 512; for
+// dh = 64 and 80 also a grid of (N / 128) x H x B CTAs of at least half the SM count).
 bool attn_wgmma_shape_ok(int B, int H, int N, int M, int dh);
 // forward: O, LSE.  backward: dK, dV, and dQ reduced into the zeroed a.dQacc (the caller converts it to bf16).
 int attn_wgmma_fwd(const AttnArgs& a, cudaStream_t st);

@@ -1,15 +1,16 @@
-// e4t — warpgroup-level attention for the long non-causal self-attention of the SD-v1.4 UNet: level 0 (N = M = 4096,
-// 8 heads of 40) and level 1 (N = M = 1024, 8 heads of 80).  wgmma.mma_async from SWIZZLE_128B shared-memory tiles
+// e4t — warpgroup-level attention for the long non-causal self-attention of the SD-v1.4 UNet, level 0 (N = M = 4096,
+// 8 heads of 40) and level 1 (N = M = 1024, 8 heads of 80), and of the SD 2.x UNet (heads of 64 at every level: 5, 10
+// and 20 heads, 9216 / 2304 / 576 tokens at 768²).  wgmma.mma_async from SWIZZLE_128B shared-memory tiles
 // that TMA fills, fp32 accumulators in registers.  Same function, arguments and outputs as the mma.sync kernels of
 // attention.cu, which keep every other shape.
 //
-// Which shapes run here (attn_wgmma_shape_ok): dh = 40 or 80, N and M multiples of 128 and >= 512; for dh = 80 also a
-// grid of (N / 128) x H x B CTAs of at least half the device's SM count.
+// Which shapes run here (attn_wgmma_shape_ok): dh = 40, 64 or 80, N and M multiples of 128 and >= 512; for dh = 64 and
+// 80 also a grid of (N / 128) x H x B CTAs of at least half the device's SM count.
 //
 // Loading: a head slice is dh bf16 wide inside a token row.  Q/K/V/dO are described to TMA as the 4-D tensor
 // (dh, H, tokens, B) with a box of 64 x 1 x rows x 1, loaded once per 64-column panel (x = 0, and x = 64 for dh = 80):
 // columns >= dh are out of bounds and arrive as zeros, so a panel is rows x 128 B, swizzled, with no neighbouring head
-// in the padding.  A tile is its panels one after the other.  Products over the head dim take ceil(dh / 16) k-steps,
+// in the padding (dh = 64 fills its panel, no padding).  A tile is its panels one after the other.  Products over the head dim take ceil(dh / 16) k-steps,
 // the fifth one (dh = 80) reading the second panel; products whose N is the head dim use an instruction of exactly
 // N = dh, which reads an MN-major operand's second panel at the descriptor's leading byte offset.
 //
@@ -468,11 +469,14 @@ attn_wgmma_bwd_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
 // Host
 // =============================================================================================
 bool attn_wgmma_shape_ok(int B, int H, int N, int M, int dh) {
-  if (!(dh == 40 || dh == 80) || N < 512 || M < 512 || N % 128 != 0 || M % 128 != 0) return false;
+  if (!(dh == 40 || dh == 64 || dh == 80) || N < 512 || M < 512 || N % 128 != 0 || M % 128 != 0) return false;
   if (dh == 40) return true;
   // dh = 80: the wgmma kernels measured faster than mma.sync at every grid down to 64 CTAs (level 1 at B = 1), so the
   // boundary is not a speed one: grids below half the SM count (that one included, on 132 SMs) keep the mma.sync
-  // kernels, and with them a level-1 shape on which those kernels stay checked against the switch
+  // kernels, and with them a level-1 shape on which those kernels stay checked against the switch.
+  // dh = 64 takes the same rule: the wgmma kernels measured faster at every SD 2.x grid down to its smallest, 80 CTAs
+  // (level 1 at 512², B = 1: forward 1.6x, backward 2.4x on an H100 SXM at 700 W; DESIGN.md §5), and every SD 2.x
+  // UNet self-attention of 512 tokens or more has at least that grid, so only smaller grids stay on mma.sync
   int sms = 0, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -497,8 +501,10 @@ int attn_wgmma_fwd(const AttnArgs& a, cudaStream_t st) {
   if (int e = head_map(&mK, a.K, a, a.M, a.ldk, a.k_bs, 128)) return e;
   if (int e = head_map(&mV, a.V, a, a.M, a.ldv, a.v_bs, 128)) return e;
   E4T_CHECK(a.ldo % 2 == 0 && a.o_bs % 2 == 0, "attention (wgmma): output strides must be even");
-  const size_t smem = a.dh == 40 ? FwdSmem<40>::bytes : FwdSmem<80>::bytes;
-  auto kernel = a.dh == 40 ? attn_wgmma_fwd_kernel<40> : attn_wgmma_fwd_kernel<80>;
+  const size_t smem = a.dh == 40 ? FwdSmem<40>::bytes : a.dh == 64 ? FwdSmem<64>::bytes : FwdSmem<80>::bytes;
+  auto kernel = a.dh == 40   ? attn_wgmma_fwd_kernel<40>
+                : a.dh == 64 ? attn_wgmma_fwd_kernel<64>
+                             : attn_wgmma_fwd_kernel<80>;
   E4T_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<dim3(a.N / 128, a.H, a.B), kWgThreads, smem, st>>>(mQ, mK, mV, a);
   E4T_COUNT_LAUNCH();
@@ -523,8 +529,10 @@ int attn_wgmma_bwd(const AttnArgs& a, cudaStream_t st) {
   }
   E4T_CHECK(a.lddk % 2 == 0 && a.dk_bs % 2 == 0 && a.lddv % 2 == 0 && a.dv_bs % 2 == 0,
             "attention (wgmma): gradient strides must be even");
-  const size_t smem = a.dh == 40 ? BwdSmem<40>::bytes : BwdSmem<80>::bytes;
-  auto kernel = a.dh == 40 ? attn_wgmma_bwd_kernel<40> : attn_wgmma_bwd_kernel<80>;
+  const size_t smem = a.dh == 40 ? BwdSmem<40>::bytes : a.dh == 64 ? BwdSmem<64>::bytes : BwdSmem<80>::bytes;
+  auto kernel = a.dh == 40   ? attn_wgmma_bwd_kernel<40>
+                : a.dh == 64 ? attn_wgmma_bwd_kernel<64>
+                             : attn_wgmma_bwd_kernel<80>;
   E4T_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kernel<<<dim3(a.M / 128, a.H, a.B), kWgThreads, smem, st>>>(mQ, mK, mV, mdO, mdQ, a);
   E4T_COUNT_LAUNCH();

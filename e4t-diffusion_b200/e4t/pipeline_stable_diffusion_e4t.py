@@ -14,7 +14,7 @@ denoising step — only the pooled UNet features do — so they are computed ONC
 instead of once per step (SURVEY.md §8 f-2).
 
 diffusers is not a dependency: the SD-v1.x DDIM scheduler (scaled-linear betas, steps_offset 1, no sample clipping,
-eta) is `DDIMScheduler` below; any object with set_timesteps / scale_model_input / step(...).prev_sample works.
+eta; epsilon or, for SD 2.x, v prediction) is `DDIMScheduler` below; any object with set_timesteps / scale_model_input / step(...).prev_sample works.
 VAE decoding (decode_latents) calls `vae.decode(z).sample` as the reference does: attach e4t's AutoencoderKL
 (e4t/models/autoencoder_kl.py, the SD VAE on the same sm_90a kernels) and `output_type="np"` / `"pil"` run end to end on
 them; with `vae=None` the pipeline can only return latents (`output_type="latent"`)."""
@@ -40,19 +40,49 @@ class _StepOutput(BaseOutput):
 
 class DDIMScheduler:
     """diffusers 0.14 DDIMScheduler as configured by SD-v1.x (scheduler/scheduler_config.json): scaled_linear betas
-    0.00085..0.012, 1000 train steps, clip_sample False, set_alpha_to_one False, steps_offset 1, epsilon prediction."""
+    0.00085..0.012, 1000 train steps, clip_sample False, set_alpha_to_one False, steps_offset 1, epsilon prediction.
+    prediction_type="v_prediction" is the SD 2.x 768-v configuration: the model predicts v = √ᾱ_t·ε − √(1−ᾱ_t)·x₀."""
     order = 1
     init_noise_sigma = 1.0
 
     def __init__(self, num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, steps_offset=1,
-                 set_alpha_to_one=False):
+                 set_alpha_to_one=False, prediction_type="epsilon"):
+        if prediction_type not in ("epsilon", "v_prediction"):
+            raise ValueError(f"prediction_type must be 'epsilon' or 'v_prediction', got {prediction_type!r}")
         betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps, dtype=torch.float32) ** 2
         self.alphas_cumprod = torch.cumprod(1.0 - betas, dim=0)
         self.final_alpha_cumprod = torch.tensor(1.0) if set_alpha_to_one else self.alphas_cumprod[0]
         self.num_train_timesteps = num_train_timesteps
         self.steps_offset = steps_offset
+        self.prediction_type = prediction_type
         self.num_inference_steps = None
         self.timesteps = torch.arange(num_train_timesteps - 1, -1, -1)
+
+    # scheduler_config.json keys this class follows; the others must hold the values it implements
+    _CONFIG_KEYS = ("num_train_timesteps", "beta_start", "beta_end", "steps_offset", "set_alpha_to_one",
+                    "prediction_type")
+
+    @classmethod
+    def from_config(cls, config):
+        """DDIMScheduler from a diffusers scheduler config (a dict, e.g. a model's scheduler_config.json).  Only the
+        scaled_linear beta schedule without sample clipping is implemented; any other is refused."""
+        if config.get("beta_schedule", "scaled_linear") != "scaled_linear":
+            raise ValueError(f"beta_schedule {config['beta_schedule']!r} is not supported (only 'scaled_linear')")
+        if config.get("clip_sample", False):
+            raise ValueError("clip_sample=True is not supported")
+        return cls(**{k: config[k] for k in cls._CONFIG_KEYS if k in config})
+
+    @classmethod
+    def from_pretrained(cls, pretrained_model_name_or_path, subfolder=None, **kw):
+        """DDIMScheduler.from_pretrained(path, subfolder="scheduler") on a local model directory (inference.py:118);
+        nothing is downloaded."""
+        import json
+        import os
+        d = os.path.join(pretrained_model_name_or_path, subfolder) if subfolder else pretrained_model_name_or_path
+        with open(os.path.join(d, "scheduler_config.json")) as f:
+            config = json.load(f)
+        config.update(kw)
+        return cls.from_config(config)
 
     def set_timesteps(self, num_inference_steps, device=None):
         self.num_inference_steps = num_inference_steps
@@ -68,9 +98,14 @@ class DDIMScheduler:
         prev_t = t - self.num_train_timesteps // self.num_inference_steps
         a_t = self.alphas_cumprod[t].to(sample.device)
         a_prev = (self.alphas_cumprod[prev_t] if prev_t >= 0 else self.final_alpha_cumprod).to(sample.device)
-        eps = model_output.to(torch.float32)
+        out = model_output.to(torch.float32)
         x = sample.to(torch.float32)
-        pred_x0 = (x - (1 - a_t) ** 0.5 * eps) / a_t ** 0.5
+        if self.prediction_type == "epsilon":
+            eps = out
+            pred_x0 = (x - (1 - a_t) ** 0.5 * eps) / a_t ** 0.5
+        else:
+            pred_x0 = a_t ** 0.5 * x - (1 - a_t) ** 0.5 * out
+            eps = a_t ** 0.5 * out + (1 - a_t) ** 0.5 * x
         var = (1 - a_prev) / (1 - a_t) * (1 - a_t / a_prev)
         std = eta * var ** 0.5
         prev = a_prev ** 0.5 * pred_x0 + (1 - a_prev - std ** 2) ** 0.5 * eps

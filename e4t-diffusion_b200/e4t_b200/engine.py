@@ -33,6 +33,24 @@ def add_noise(latents, noise, timesteps, acp):
     return a.view(-1, 1, 1, 1) * latents + s.view(-1, 1, 1, 1) * noise
 
 
+def get_velocity(latents, noise, timesteps, acp):
+    """diffusers 0.14 DDPMScheduler.get_velocity: the v-prediction target √ᾱ_t·noise − √(1−ᾱ_t)·latents, indexed as
+    add_noise is."""
+    a = acp[timesteps] ** 0.5
+    s = (1 - acp[timesteps]) ** 0.5
+    return a.view(-1, 1, 1, 1) * noise - s.view(-1, 1, 1, 1) * latents
+
+
+PREDICTION_TYPES = ("epsilon", "v_prediction")
+
+
+def check_prediction_type(prediction_type):
+    """noise_scheduler.config.prediction_type of the base model (pretrain_e4t.py:638-643, tuning_e4t.py:318-323)."""
+    if prediction_type not in PREDICTION_TYPES:
+        raise ValueError(f"prediction_type must be 'epsilon' or 'v_prediction', got {prediction_type!r}")
+    return prediction_type
+
+
 def all_reduce_sum_(flat, group=None):
     """Data-parallel exchange of a flat gradient arena: ONE all-reduce(SUM) (NCCL over NVLink/NVSwitch on GPUs,
     gloo in the CPU tests).  Returns the scale (1/world) that turns the sum into the DDP average; FlatAdamW folds it
@@ -228,10 +246,14 @@ class PretrainStep:
                  betas=(0.9, 0.999), weight_decay=1e-2, eps=1e-8, domain_embed_scale=0.1, reg_lambda=0.01,
                  bos_id=49406, eos_id=49407, weight_dtype=torch.bfloat16, optimizer=True, tune_unet=False,
                  max_grad_norm=None, vae=None, train_text_encoder=False, use_8bit_adam=False, lr_scheduler="constant",
-                 lr_warmup_steps=0, max_train_steps=None):
+                 lr_warmup_steps=0, max_train_steps=None, prediction_type="epsilon", pad_id=49407):
         # use_8bit_adam / lr_scheduler / lr_warmup_steps / max_train_steps: the optimiser flags of pretrain_e4t.py and
         # tuning_e4t.py (FlatAdamW); refused before anything is built
         optim.check_schedule(lr_scheduler, lr_warmup_steps, max_train_steps, lr)
+        # prediction_type: the base model's noise_scheduler.config.prediction_type ("v_prediction" for the SD 2.x 768-v
+        # models); pad_id: the tokenizer's pad token, which fills the empty prompt after [BOS, EOS] (49407 for SD 1.x,
+        # 0 for the SD 2.x tokenizer)
+        self.prediction_type = check_prediction_type(prediction_type)
         self.unet, self.enc, self.text = unet, e4t_encoder, text_encoder
         # vae: an e4t AutoencoderKL; with it, a batch without "latents" is encoded on the device (pretrain_e4t.py:598-599)
         self.vae = vae
@@ -251,7 +273,7 @@ class PretrainStep:
             raise ValueError("train_text_encoder needs fp32 text-encoder weights (tuning_e4t.py --train_text_encoder)")
         self.text.requires_grad_(self.train_text_encoder)                                # pretrain_e4t.py:262-263
         self.class_ids = torch.tensor([class_token_id], device=dev)
-        self.ids_e4t = torch.tensor([[bos_id] + [eos_id] * 76], device=dev)
+        self.ids_e4t = torch.tensor([[bos_id, eos_id] + [pad_id] * 75], device=dev)
         self.class_embed, self.ehs_e4t = self._text_constants()
         # tune_unet / max_grad_norm: the domain-tuning step (tuning_e4t.py:270-338): every UNet weight trainable,
         # global gradient-norm clipping over UNet + encoder parameters (:329-335)
@@ -349,7 +371,11 @@ class PretrainStep:
         inputs_embeds = inputs_embeds.to(domain_embed.dtype).index_put((rows, cols), domain_embed)
         ehs = self.text(inputs_embeds=inputs_embeds.to(self.text.dtype))[0].to(self.weight_dtype)        # :634
         pred = self.unet(noisy, timesteps, ehs).sample                                   # :636
-        loss_diff = F.mse_loss(pred.float(), noise.float(), reduction="mean")            # :645
+        if self.prediction_type == "epsilon":                                            # :638-643
+            target = noise
+        else:
+            target = get_velocity(latents, noise, timesteps, self.acp)
+        loss_diff = F.mse_loss(pred.float(), target.float(), reduction="mean")           # :645
         loss_reg = self.reg_lambda * domain_embed.pow(2).sum()                           # :646
         return dict(loss=loss_diff + loss_reg, loss_diff=loss_diff, loss_reg=loss_reg, pred=pred,
                     domain_embed=domain_embed, placeholder_idxs=idxs)

@@ -419,9 +419,9 @@ def _bs(t):
 def attn_fwd(q, k, v, heads, scale=None):
     """q (B,N,H*dh), k/v (B,M,H*dh) bf16 (last dim contiguous; may be column slices of a fused projection).
     Returns (o (B,N,H*dh) bf16, lse (B,H,N) fp32).
-    dh == 40 or 80 with N and M multiples of 128, >= 512 (the 4096-token and 1024-token self-attention; for dh == 80
-    only grids of at least half as many 128-query CTAs as SMs) runs the warpgroup (wgmma + TMA) kernel; every other shape, or
-    E4T_ATTN_WGMMA=0, the mma.sync kernel."""
+    dh == 40, 64 or 80 with N and M multiples of 128, >= 512 (the SD 1.x 4096-token and 1024-token self-attention, the
+    SD 2.x self-attention with heads of 64; for dh == 64 and 80 only grids of at least half as many 128-query CTAs as
+    SMs) runs the warpgroup (wgmma + TMA) kernel; every other shape, or E4T_ATTN_WGMMA=0, the mma.sync kernel."""
     assert q.dtype == BF16 and k.dtype == BF16 and v.dtype == BF16
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1
     Bn, N, C = q.shape
