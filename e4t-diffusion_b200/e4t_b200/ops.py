@@ -410,6 +410,49 @@ def adamw8bit_step_sched(p, g, m_codes, v_codes, m_absmax, v_absmax, qmap_m, qma
 
 
 # ----------------------------------------------------------------------------------------------
+# sampling: one scheduler update from a coefficient table (e4t/schedulers.py)
+# ----------------------------------------------------------------------------------------------
+def sampler_history_buffer(n_hist, n, device):
+    """History slots for `sampler_step`: (n_hist, n rounded up to 4) fp32, so every slot starts 16-byte aligned."""
+    return torch.zeros(n_hist, (n + 3) // 4 * 4, dtype=F32, device=device)
+
+
+def _need(cond, msg):
+    if not cond:
+        raise _lib.E4TError(f"sampler_step: {msg}")
+
+
+def sampler_step(out, x, x_next, hist, saved, noise, table, step_dev, row, guidance=None, t_out=None, model_in=None):
+    """e4t_sampler_step: publish row *step_dev of `table` into `row`, advance the counter and apply the row to the n
+    elements of `x`, writing `x_next` (may be `x`), the history slot, the saved sample and, when given, the next step's
+    model input (all G rows) and timestep.  `out` holds n (no guidance) or 2n (uncond rows first; `guidance` is then a
+    1-element fp32 device tensor) elements.  Every check runs before any launch."""
+    n = x.numel()
+    bufs = dict(out=out, x=x, x_next=x_next, saved=saved, row=row, noise=noise, t_out=t_out, model_in=model_in,
+                guidance=guidance, hist=hist)
+    for k, t in bufs.items():
+        if t is None:
+            continue
+        _need(t.is_cuda and t.dtype == F32 and t.is_contiguous(), f"{k} must be a contiguous fp32 CUDA tensor")
+    _need(n > 0 and out.numel() in (n, 2 * n), f"out has {out.numel()} elements for {n} latents (need n or 2n)")
+    G = out.numel() // n
+    _need(G == 1 or (guidance is not None and guidance.numel() == 1), "guidance (1 element) is needed with 2n outputs")
+    _need(x_next.numel() == n and saved.numel() == n and (noise is None or noise.numel() == n),
+          "x_next, saved and noise must have as many elements as x")
+    _need(model_in is None or model_in.numel() == G * n, f"model_in must have {G} x {n} elements")
+    _need(t_out is None or t_out.numel() == 1, "t_out must have 1 element")
+    _need(hist.dim() == 2 and hist.shape[0] <= 4 and (hist.shape[0] == 0 or hist.shape[1] >= n),
+          "hist must be (slots <= 4, >= n)")
+    _need(table.is_cuda and table.dtype == torch.float64 and table.is_contiguous() and table.dim() == 2
+          and table.shape[1] == 14 and table.shape[0] >= 1, "table must be a contiguous (rows >= 1, 14) fp64 CUDA tensor")
+    _need(step_dev.is_cuda and step_dev.dtype == torch.int32 and step_dev.numel() == 1, "step_dev must be 1 int32")
+    _need(row.numel() >= 14, "row needs 14 elements")
+    _lib.call("e4t_sampler_step", ptr(out), c_int(G), ptr(guidance), ptr(x), ptr(x_next), ptr(hist),
+              c_int(hist.shape[0]), c_ll(hist.shape[1]), ptr(saved), ptr(noise), ptr(table), c_int(table.shape[0]),
+              ptr(step_dev), ptr(row), ptr(t_out), ptr(model_in), c_ll(n), stream())
+
+
+# ----------------------------------------------------------------------------------------------
 # attention core
 # ----------------------------------------------------------------------------------------------
 def _bs(t):

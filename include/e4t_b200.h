@@ -229,6 +229,19 @@ int e4t_adamw8bit_step_sched(float* p, const float* g, unsigned char* m_codes, u
                              int sched_kind, int warmup, int total, double num_cycles, double power, double lr_end,
                              float grad_scale, void* stream);
 
+/* ---- sampling (scheduler.step at pipeline_stable_diffusion_e4t.py:211-216, inference.py --scheduler_type) ------------
+ * One denoising update from a coefficient table (format: e4t/schedulers.py; one fp64 row of 14 per step, n_rows rows).
+ * A tick publishes row min(*step_dev, n_rows - 1) as fp32 into row[14], writes its next-step timestep to *t_out (the
+ * UNet's fp32 timestep buffer; may be NULL) and increments *step_dev; the update then, per element of the n latents:
+ *   e = out (G = 1) or u + g·(c − u) with u = out[0][j], c = out[1][j], g = *guidance (G = 2, uncond rows first);
+ *   x_next = r[0]·x + r[1]·e + Σ_k r[2+k]·hist[k] + r[6]·saved + r[7]·noise;
+ *   hist[r[8]] = r[9]·x + r[10]·e (r[8] >= 0); saved = x (r[11] != 0); model_in[g][j] = r[12]·x_next for g < G.
+ * out [G][n], x / x_next (may alias) / saved / noise [n] fp32; hist [n_hist <= 4][hist_ld]; noise and model_in may be
+ * NULL.  fp32 arithmetic, float4 accesses when every buffer allows them, a scalar tail, no atomics. */
+int e4t_sampler_step(const float* out, int G, const float* guidance, const float* x, float* x_next, float* hist,
+                     int n_hist, long long hist_ld, float* saved, const float* noise, const double* table, int n_rows,
+                     int* step_dev, float* row, float* t_out, float* model_in, long long n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
