@@ -63,20 +63,50 @@ class BasicTransformerBlock(nn.Module):
         self.norm2 = nn.LayerNorm(dim, elementwise_affine=norm_elementwise_affine) if self.attn2 is not None else None
         self.norm3 = nn.LayerNorm(dim, elementwise_affine=norm_elementwise_affine)
 
+    _tome = None   # the token-merging patch in force (e4t_b200.tome.apply_patch), shared by the UNet's blocks
+
     @staticmethod
     def _ln(norm, x):
         return FN.LayerNormFn.apply(x, norm.weight, norm.bias, norm.eps)
 
     def forward(self, hidden_states, encoder_hidden_states=None, timestep=None, attention_mask=None,
-                cross_attention_kwargs=None, class_labels=None):
+                cross_attention_kwargs=None, class_labels=None, hw=None):
+        """hw: the (H, W) grid of the tokens, which token merging needs (Transformer2DModel passes it)."""
         kw = cross_attention_kwargs if cross_attention_kwargs is not None else {}
         x = FN.as_bf16(hidden_states)
+        if self._tome is not None and hw is not None:
+            from e4t_b200 import tome
+            plan = tome.plan(self._tome, x, hw)
+            if plan is not None:
+                return self._forward_merged(x, plan, self._tome["args"], encoder_hidden_states, attention_mask, kw)
         x = self.attn1(self._ln(self.norm1, x), encoder_hidden_states=None, attention_mask=attention_mask,
                        residual=x, **kw)                                                   # attention.py:291-302
         if self.attn2 is not None:
             x = self.attn2(self._ln(self.norm2, x), encoder_hidden_states=encoder_hidden_states,
                            attention_mask=attention_mask, residual=x, **kw)                # :304-316
         return self.ff(self._ln(self.norm3, x), residual=x)                                # :318-330
+
+    def _forward_merged(self, x, plan, a, encoder_hidden_states, attention_mask, kw):
+        """tomesd's patched block: each sub-layer that merges runs on the N - r merged tokens and is unmerged with the
+        residual added by the same kernel (its out-projection then runs without the fused residual)."""
+        if a.merge_attn:
+            h = FN.ToMeMergeFn.apply(self._ln(self.norm1, x), plan)
+            x = FN.ToMeUnmergeFn.apply(self.attn1(h, encoder_hidden_states=None, attention_mask=attention_mask, **kw),
+                                       plan, x)
+        else:
+            x = self.attn1(self._ln(self.norm1, x), encoder_hidden_states=None, attention_mask=attention_mask,
+                           residual=x, **kw)
+        if self.attn2 is not None:
+            if a.merge_crossattn:
+                h = FN.ToMeMergeFn.apply(self._ln(self.norm2, x), plan)
+                x = FN.ToMeUnmergeFn.apply(self.attn2(h, encoder_hidden_states=encoder_hidden_states,
+                                                      attention_mask=attention_mask, **kw), plan, x)
+            else:
+                x = self.attn2(self._ln(self.norm2, x), encoder_hidden_states=encoder_hidden_states,
+                               attention_mask=attention_mask, residual=x, **kw)
+        if a.merge_mlp:
+            return FN.ToMeUnmergeFn.apply(self.ff(FN.ToMeMergeFn.apply(self._ln(self.norm3, x), plan)), plan, x)
+        return self.ff(self._ln(self.norm3, x), residual=x)
 
 
 # the fp32 score matrix of one image is N² · 4 bytes (64 MiB at a 64 x 64 latent); images are processed in chunks

@@ -74,7 +74,7 @@ class Transformer2DModel(ModelMixin, ConfigMixin):
                               self.proj_in.weight)                                                   # :253-261
         for block in self.transformer_blocks:                                                           # :268-275
             h = block(h, encoder_hidden_states=encoder_hidden_states, timestep=timestep,
-                      cross_attention_kwargs=cross_attention_kwargs, class_labels=class_labels)
+                      cross_attention_kwargs=cross_attention_kwargs, class_labels=class_labels, hw=(H, W))
         out = FN.LinearFn.apply(h, self._w(self.proj_out), self.proj_out.bias, x.view(B, H * W, C),
                                 self.proj_out.weight)                                                # :279-286
         out = out.view(B, H, W, C)

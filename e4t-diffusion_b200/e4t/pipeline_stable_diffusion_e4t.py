@@ -246,8 +246,9 @@ class StableDiffusionE4TPipeline:
         """The denoising loop as T replays of one captured step.  Prologue (eager): the table upload, the counter
         reset, the first scaled model input and timestep, and the per-call data (prompt embeddings, placeholder index,
         image features, guidance and domain scales) copied into the static buffers.  The graph is keyed by shapes,
-        guidance on / off, dtypes and the scheduler's history slot count only."""
+        guidance on / off, dtypes, the scheduler's history slot count, the parameters and the token-merging patch."""
         from e4t.schedulers import Z
+        from e4t_b200 import tome
         sched = self.scheduler
         if not hasattr(sched, "sampler_table"):
             raise ValueError(f"the CUDA-graph sampling path needs a scheduler with sampler_table(); "
@@ -265,7 +266,8 @@ class StableDiffusionE4TPipeline:
                                                                            device=device)
         key = (tuple(latents.shape), latents.dtype, cfg, self.unet.dtype, self.text_encoder.dtype,
                int(sched.sampler_history), tuple(base_emb.shape), tuple(ehs_e4t.shape), tuple(pixel_values.shape),
-               tuple(tuple(f.shape) for f in clip_feats), str(device), self._param_signature())
+               tuple(tuple(f.shape) for f in clip_feats), str(device), self._param_signature(),
+               tome.signature(self.unet))
         data = dict(x=latents, t=timesteps[0], base_emb=base_emb, idx=e4t["placeholder_token_id_idx"],
                     ehs_e4t=ehs_e4t, pix=pixel_values, clip=clip_feats, class_embed=class_embed,
                     guidance=guidance_scale, dscale=domain_embed_scale, table=table,

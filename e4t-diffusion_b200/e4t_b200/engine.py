@@ -16,6 +16,7 @@ import torch.nn.functional as F
 from . import functional as FN
 from . import ops
 from . import optim
+from . import tome
 from ._lib import E4TError
 
 PLACEHOLDER_FALLBACK = 49408
@@ -285,6 +286,7 @@ class PretrainStep:
                              lr_warmup_steps=lr_warmup_steps, max_train_steps=max_train_steps,
                              optim_bits=8 if use_8bit_adam else 32) if optimizer else None
         self._graph = None
+        self._graph_tome = None
         self.wo_bank = None
         self._wo_factor_exchange = False
         # Data parallel: the encoder-head gradients (925 MB of the 1.5 GB arena, an arena prefix) are final as soon as
@@ -442,6 +444,7 @@ class PretrainStep:
             graph = capture(self._eager_step, "global")
         self._drop_autograd_refs()
         self._graph = graph
+        self._graph_tome = tome.signature(self.unet)
         return self
 
     def _disable_wo_factor_exchange(self):
@@ -473,6 +476,9 @@ class PretrainStep:
 
     def __call__(self, batch):
         if self._graph is not None:
+            if tome.signature(self.unet) != self._graph_tome:
+                raise E4TError("the UNet's token-merging patch changed after enable_cuda_graph(): the captured step "
+                               "would replay the old one; call release_cuda_graph() and capture again")
             for k, v in batch.items():
                 self._static[k].copy_(v, non_blocking=True)
             self._graph.replay()

@@ -678,3 +678,34 @@ class MeanPoolCatFn(torch.autograd.Function):
             outs.append(ops.meanpool_bwd(dout, shp, off) if ctx.needs_input_grad[i] else None)
             off += shp[-1]
         return tuple(outs)
+
+
+# ----------------------------------------------------------------------------------------------
+# token merging (e4t_b200/tome.py): both maps are linear in the tokens; the plan (matching) carries no gradient
+# ----------------------------------------------------------------------------------------------
+class ToMeMergeFn(torch.autograd.Function):
+    """(B, N, C) -> (B, N', C): each merged row is the mean of its members.  Backward: dx[i] = dy[pos i] / len."""
+
+    @staticmethod
+    def forward(ctx, x, plan):
+        ctx.plan = plan
+        return ops.tome_gather_reduce(_c(as_bf16(x)), plan, weighted=True)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return ops.tome_gather_expand(_c(dy), ctx.plan, weighted=True), None
+
+
+class ToMeUnmergeFn(torch.autograd.Function):
+    """(B, N', C) -> (B, N, C): out[i] = y[pos i] + residual[i].  Backward: dy[p] = sum of dout over row p's
+    members; dresidual = dout."""
+
+    @staticmethod
+    def forward(ctx, y, plan, residual):
+        ctx.plan = plan
+        return ops.tome_gather_expand(_c(y), plan, weighted=False, residual=_c(residual))
+
+    @staticmethod
+    def backward(ctx, dout):
+        dout = _c(dout)
+        return ops.tome_gather_reduce(dout, ctx.plan, weighted=False), None, dout

@@ -634,3 +634,94 @@ def conv3x3_wgrad(x, dy):
     _lib.call("e4t_conv3x3_wgrad", ptr(x), ptr(dy), ptr(dw9), c_int(Bn), c_int(H), c_int(W), c_int(Cin), c_int(Cout),
               stream())
     return dw9
+
+
+# ----------------------------------------------------------------------------------------------
+# token merging (csrc/tome.cu)
+# ----------------------------------------------------------------------------------------------
+TOME_MAX_TOKENS = 16384   # tokens per image the select kernel takes (a 128 x 128 latent)
+
+
+def _tome_need(cond, msg):
+    if not cond:
+        raise _lib.E4TError(f"token merging: {msg}")
+
+
+def tome_match(x, pattern, h, w, sy, sx):
+    """Bipartite matching of x (B, h*w, C) bf16 (C % 64 == 0): one dst token per sy x sx cell at offset pattern[cy, cx]
+    (int32 (h // sy, w // sx) CUDA tensor), every other token src.  Returns dict(slot (N,), src_idx (Ns,), dst_idx
+    (Nd,), node_max (B, Ns) fp32, node_idx (B, Ns) int32 raster index of the best dst)."""
+    _tome_need(x.is_cuda and x.dtype == BF16 and x.dim() == 3 and x.is_contiguous(), "x must be a contiguous (B, N, C) "
+               "bf16 CUDA tensor")
+    Bn, N, C = x.shape
+    _tome_need(h > 0 and w > 0 and h * w == N, f"{N} tokens are not an {h} x {w} grid")
+    _tome_need(C % 64 == 0, f"C = {C} is not a multiple of 64")
+    _tome_need(sy >= 1 and sx >= 1, f"stride ({sy}, {sx}) must be >= 1")
+    hc, wc = h // sy, w // sx
+    _tome_need(pattern.is_cuda and pattern.dtype == torch.int32 and pattern.is_contiguous()
+               and tuple(pattern.shape) == (hc, wc), f"pattern must be a contiguous int32 ({hc}, {wc}) CUDA tensor")
+    Nd = hc * wc
+    Ns = N - Nd
+    i32 = dict(device=x.device, dtype=torch.int32)
+    slot, src_idx, dst_idx = torch.empty(N, **i32), torch.empty(max(Ns, 1), **i32), torch.empty(max(Nd, 1), **i32)
+    src_n = torch.empty((Bn, max(Ns, 1), C), device=x.device, dtype=BF16)
+    dst_n = torch.empty((Bn, max(Nd, 1), C), device=x.device, dtype=BF16)
+    node_max = torch.empty((Bn, Ns), device=x.device, dtype=F32)
+    node_idx = torch.empty((Bn, Ns), **i32)
+    _lib.call("e4t_tome_match", ptr(x), ptr(pattern), c_int(Bn), c_int(h), c_int(w), c_int(C), c_int(sy), c_int(sx),
+              ptr(slot), ptr(src_idx), ptr(dst_idx), ptr(src_n), ptr(dst_n), ptr(node_max), ptr(node_idx), stream())
+    return dict(slot=slot, src_idx=src_idx[:Ns], dst_idx=dst_idx[:Nd], node_max=node_max, node_idx=node_idx)
+
+
+def tome_select(m, r):
+    """Merge the r src tokens of each image with the largest node_max (ties to the lower raster index) given
+    tome_match's result `m`.  Returns dict(pos (B, N), row_off (B, N - r + 1), members (B, N) int32, w (B, N - r)
+    fp32 = 1 / row length)."""
+    Bn, Ns = m["node_max"].shape
+    N, Nd = m["slot"].numel(), m["dst_idx"].numel()
+    _tome_need(N <= TOME_MAX_TOKENS, f"{N} tokens per image; the select kernel takes at most {TOME_MAX_TOKENS} "
+               "(a 128 x 128 latent)")
+    _tome_need(0 <= r <= Ns and (r == 0 or Nd > 0), f"r = {r} with {Ns} src and {Nd} dst tokens")
+    dev = m["slot"].device
+    i32 = dict(device=dev, dtype=torch.int32)
+    seg = torch.empty((Bn, 2, max(Nd, 1)), **i32)
+    pos, members = torch.empty((Bn, N), **i32), torch.empty((Bn, N), **i32)
+    row_off = torch.empty((Bn, N - r + 1), **i32)
+    w = torch.empty((Bn, N - r), device=dev, dtype=F32)
+    _lib.call("e4t_tome_select", ptr(m["node_max"]), ptr(m["node_idx"]), ptr(m["slot"]), ptr(m["src_idx"]), c_int(Bn),
+              c_int(N), c_int(Ns), c_int(Nd), c_int(r), ptr(seg), ptr(pos), ptr(row_off), ptr(members), ptr(w),
+              stream())
+    return dict(pos=pos, row_off=row_off, members=members, w=w)
+
+
+def _tome_rows(t, name, Bn, n, C):
+    _tome_need(t.is_cuda and t.dtype == BF16 and t.is_contiguous() and tuple(t.shape) == (Bn, n, C),
+               f"{name} must be a contiguous bf16 ({Bn}, {n}, {C}) CUDA tensor, got {tuple(t.shape)} {t.dtype}")
+
+
+def tome_gather_reduce(x, plan, weighted):
+    """(B, N, C) -> (B, N', C): row p = (1 / len if weighted else 1) * sum of x over the members of merged row p."""
+    Bn, N = plan["pos"].shape
+    Nm = plan["w"].shape[1]
+    C = x.shape[-1]
+    _tome_rows(x, "x", Bn, N, C)
+    _tome_need(C % 8 == 0, f"C = {C} is not a multiple of 8")
+    out = torch.empty((Bn, Nm, C), device=x.device, dtype=BF16)
+    _lib.call("e4t_tome_gather_reduce", ptr(x), ptr(plan["row_off"]), ptr(plan["members"]),
+              ptr(plan["w"] if weighted else None), ptr(out), c_int(Bn), c_int(N), c_int(Nm), c_int(C), stream())
+    return out
+
+
+def tome_gather_expand(y, plan, weighted, residual=None):
+    """(B, N', C) -> (B, N, C): out[i] = (w[pos i] if weighted else 1) * y[pos i] (+ residual[i])."""
+    Bn, N = plan["pos"].shape
+    Nm = plan["w"].shape[1]
+    C = y.shape[-1]
+    _tome_rows(y, "y", Bn, Nm, C)
+    _tome_need(C % 8 == 0, f"C = {C} is not a multiple of 8")
+    if residual is not None:
+        _tome_rows(residual, "residual", Bn, N, C)
+    out = torch.empty((Bn, N, C), device=y.device, dtype=BF16)
+    _lib.call("e4t_tome_gather_expand", ptr(y), ptr(plan["pos"]), ptr(plan["w"] if weighted else None),
+              ptr(residual), ptr(out), c_int(Bn), c_int(Nm), c_int(N), c_int(C), stream())
+    return out

@@ -242,6 +242,29 @@ int e4t_sampler_step(const float* out, int G, const float* guidance, const float
                      int n_hist, long long hist_ld, float* saved, const float* noise, const double* table, int n_rows,
                      int* step_dev, float* row, float* t_out, float* model_in, long long n, void* stream);
 
+/* ---- token merging (ToMe: tomesd's bipartite_soft_matching_random2d and its patched BasicTransformerBlock) ---------
+ * Matching of x [B][h*w][C] bf16 (C % 64 == 0) with one dst token per sy x sx cell at offset pattern[cy][cx] (int32
+ * [h/sy][w/sx], shared by the batch); every other token is src.  Writes slot[N] (src rank >= 0, or -(dst rank + 1)),
+ * src_idx[Ns] / dst_idx[Nd] (raster indices, raster order), the unit-norm rows src_n [B][Ns][C] / dst_n [B][Nd][C]
+ * (bf16 scratch) and per src token node_max [B][Ns] (largest cosine similarity to a dst of its image, fp32) and
+ * node_idx [B][Ns] (raster index of that dst; ties to the lowest).  Nd = (h/sy)(w/sx), Ns = h*w - Nd. */
+int e4t_tome_match(const void* x, const int* pattern, int B, int h, int w, int C, int sy, int sx, int* slot,
+                   int* src_idx, int* dst_idx, void* src_n, void* dst_n, float* node_max, int* node_idx, void* stream);
+/* Selection of the r src tokens with the largest node_max (ties to the lower raster index), N <= 16384 tokens per
+ * image.  Writes pos [B][N] (merged row of each token's representative; kept tokens in raster order), row_off
+ * [B][N-r+1] and members [B][N] (CSR rows, members in ascending raster order) and w [B][N-r] = 1 / row length.
+ * seg: int32 scratch [B][2][Nd].  Deterministic, no atomics. */
+int e4t_tome_select(const float* node_max, const int* node_idx, const int* slot, const int* src_idx, int B, int N,
+                    int Ns, int Nd, int r, int* seg, int* pos, int* row_off, int* members, float* w, void* stream);
+/* out[b][p] = w[b][p] (1 if w is NULL) * sum over k in [row_off[p], row_off[p+1]) of in[b][members[k]]  (bf16 rows of
+ * C % 8 == 0 channels, fp32 sums in member order): the merge forward and the unmerge backward. */
+int e4t_tome_gather_reduce(const void* in, const int* row_off, const int* members, const float* w, void* out, int B,
+                           int n_in, int n_rows, int C, void* stream);
+/* out[b][i] = w[b][pos[i]] (1 if w is NULL) * in[b][pos[b][i]] (+ residual[b][i]): the unmerge forward with the
+ * block's residual add, and the merge backward. */
+int e4t_tome_gather_expand(const void* in, const int* pos, const float* w, const void* residual, void* out, int B,
+                           int n_in, int n_out, int C, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
